@@ -452,11 +452,11 @@ ht_encode_fast_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
     uint32_t rs_lo = sg_lo, rs_hi = sg_hi, rs_carry = 0;
     uint32_t cu_lo = 0, cu_hi = 0;
     uint32_t wj = gw[0], x_carry = 0;
-    uint4 na = r0[0], nb = r1[0];
+    uint4 na = ld_stream16(r0), nb = ld_stream16(r1);
     #pragma unroll 1
     for (uint32_t j = 0; j < npairs; ++j) {
       const uint4 ca = na, cb = nb;
-      if (j + 1 < npairs) { na = r0[j + 1]; nb = r1[j + 1]; }          // next pair in flight while this one is coded
+      if (j + 1 < npairs) { na = ld_stream16(r0 + j + 1); nb = ld_stream16(r1 + j + 1); }   // next pair in flight while this one is coded
       const uint32_t wj1 = gw[(j + 1) * ES_THREADS];
       const uint32_t y6 = rs_carry | ((rs_lo & 0x1Fu) << 1);
       const uint32_t z = y6 | (y6 >> 1);
@@ -636,11 +636,11 @@ ht_encode_split_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
         uint32_t rs_lo = sg_lo, rs_hi = sg_hi, rs_carry = 0;
         uint32_t cu_lo = 0, cu_hi = 0;
         uint32_t wj = gw[0], x_carry = 0;
-        uint4 na = r0[0], nb = r1[0];
+        uint4 na = ld_stream16(r0), nb = ld_stream16(r1);
         #pragma unroll 1
         for (uint32_t j = 0; j < npairs; ++j) {
           const uint4 ca = na, cb = nb;
-          if (j + 1 < npairs) { na = r0[j + 1]; nb = r1[j + 1]; }
+          if (j + 1 < npairs) { na = ld_stream16(r0 + j + 1); nb = ld_stream16(r1 + j + 1); }
           const uint32_t wj1 = gw[(j + 1) * SE_BLOCKS];
           const uint32_t y6 = rs_carry | ((rs_lo & 0x1Fu) << 1);
           const uint32_t z = y6 | (y6 >> 1);
@@ -784,8 +784,8 @@ void launch_ht_encode_serial(const EncBlock* blocks, uint32_t nblocks, uint32_t 
   cudaFuncSetAttribute(ht_encode_serial_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   dim3 grid((nblocks + ES_THREADS - 1) / ES_THREADS), block(ES_THREADS);
   if (nfast) {
-    // one thread per block by default; OJB_ENC_SPLIT=1 selects the two-thread split
-    static const bool split = [] { const char* e = getenv("OJB_ENC_SPLIT"); return e && atoi(e) != 0; }();
+    // the two-thread split by default (see launch_ht_decode_serial); OJB_ENC_SPLIT=0 selects one thread per block
+    static const bool split = [] { const char* e = getenv("OJB_ENC_SPLIT"); return !(e && *e && atoi(e) == 0); }();
     if (split) {
       dim3 g2((nblocks + SE_BLOCKS - 1) / SE_BLOCKS), b2(2 * SE_BLOCKS);
       OJB_LAUNCH(ht_encode_split_kernel, g2, b2, 0, st, blocks, nblocks, coef, slots, results, tables, status);

@@ -162,10 +162,10 @@ struct FrameInfo {
   uint32_t nlt_type[16];
 };
 
-// block-coder variants, identical results.  Encoder: one thread per code-block by default (fewest
-// instructions, best with several frames in flight), OJB_BLOCK_ENCODER=warp selects one warp per
-// block.  Decoder: the single-pass thread-per-block kernel by default, OJB_BLOCK_DECODER=twostep selects
-// step 1 (thread per block) + step 2 (warp per block).
+// block-coder variants, identical results.  Encoder: the thread-per-block family by default (blocks of the
+// common shape split over two threads, OJB_ENC_SPLIT=0 keeps them on one), OJB_BLOCK_ENCODER=warp selects one
+// warp per block.  Decoder: the same family (producer / consumer pair for the common shape, OJB_DEC_SPLIT=0 for
+// one thread), OJB_BLOCK_DECODER=twostep selects step 1 (thread per block) + step 2 (warp per block).
 bool serial_block_encoder();
 bool serial_block_decoder();
 
