@@ -65,6 +65,24 @@ def frame_for(p, kind="synth", seed=1234):
     return fr
 
 
+# 9/7: largest share of samples on which our decode of a codestream may differ (by one) from the reference's decode of
+# the same codestream, for components of up to 12 bits.  The two differ only where a float32 result lies within
+# rounding noise of a half (a tie, see tests/test_irv_precision.py); that noise is a fixed fraction of the normalised
+# sample, so the tie band, in output levels, doubles with every bit of depth.  Up to 12 bits the CPU tier shows at most
+# 0.03 % of samples, so 0.2 % leaves a margin of six; 16-bit components show up to 0.4 % against a bound of 3.2 %.
+IRV_DIFF_FRACTION = 0.002
+
+
+def assert_irv_matches_reference(ours, ref_planes, what="", bit_depths=None):
+    """our decode against the reference's decode of the same codestream, sample by sample"""
+    import numpy as np
+    for c, (a, b) in enumerate(zip(ours, ref_planes)):
+        d = np.abs(a.astype(np.int64) - b.astype(np.int64))
+        assert a.shape == b.shape and (d.size == 0 or d.max() <= 1), (what, c)
+        bound = IRV_DIFF_FRACTION * 2.0 ** max(0, (bit_depths[c] if bit_depths else 12) - 12)
+        assert (d != 0).mean() <= bound if d.size else True, (what, c, float((d != 0).mean()))
+
+
 def mse_pae(a, b):
     """per-component MSE (float) and peak absolute error (tests/mse_pae.cpp:522-567)"""
     import numpy as np

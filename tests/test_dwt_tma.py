@@ -12,7 +12,7 @@ SCRIPT = r'''
 import sys, os
 sys.path.insert(0, %(root)r); sys.path.insert(0, os.path.join(%(root)r, "tests"))
 import numpy as np
-import openjph_b200 as ob, images, refharness as R
+import openjph_b200 as ob, images, refharness as R, cases as CS
 lib = None
 if %(emu)d:
     import emu
@@ -36,6 +36,7 @@ for w, h, nc, bd, kw, st in cases:
     else:
         assert abs(len(cs) - len(want)) <= max(4, len(want) // 1000), (w, h, kw)
         out = ob.Decoder(lib=lib).decode(cs); ref, _ = R.decode(want)
+        CS.assert_irv_matches_reference(ob.Decoder(lib=lib).decode(want), ref, (w, h))
         for a, b, f in zip(out, ref, fr):          # the reference tests' tolerance: MSE within 1 %%, peak error within 1
             ma, mb = float(np.mean((a - f) ** 2.0)), float(np.mean((b - f) ** 2.0))
             assert abs(ma - mb) <= max(0.01 * mb, 0.01) and abs(int(np.abs(a - f).max()) - int(np.abs(b - f).max())) <= 1

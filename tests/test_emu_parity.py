@@ -33,6 +33,7 @@ def test_irv_within_tolerance(name, emu_lib, ref):
     out = ob.Decoder(lib=emu_lib).decode(want)
     got = ob.Encoder(p, ob.I32, lib=emu_lib).encode(frame)
     cross, _ = ref.decode(got)
+    cases.assert_irv_matches_reference(out, ref_planes, name)
     for c in range(p.num_comps):
         m_ref, p_ref = cases.mse_pae(ref_planes[c], frame[c])
         for planes in (out, cross):

@@ -35,6 +35,7 @@ def test_irv_within_tolerance(name, gpu_lib, ref):
     out = ob.Decoder().decode(want)
     got = ob.Encoder(p, ob.I32).encode(frame)
     cross, _ = ref.decode(got)
+    cases.assert_irv_matches_reference(out, ref_planes, name)
     for c in range(p.num_comps):
         m_ref, p_ref = cases.mse_pae(ref_planes[c], frame[c])
         for planes in (out, cross):
@@ -135,6 +136,7 @@ def test_cfg3_4k_12bit_irv_q90(gpu_lib, ref):
     got = ob.Encoder(p, ob.U16).encode([f.astype(np.uint16) for f in frame])
     out = ob.Decoder().decode(want, ob.U16)
     cross, _ = ref.decode(got)
+    cases.assert_irv_matches_reference(out, ref_planes, "cfg3")
     assert abs(len(got) - len(want)) <= len(want) // 1000 + 16
     for c in range(3):
         m_ref, p_ref = cases.mse_pae(ref_planes[c], frame[c])
@@ -176,6 +178,7 @@ def test_cfg5_4k_10bit_irv_frame(gpu_lib, ref):
     out = ob.Decoder().decode(want, ob.U16)
     got = ob.Encoder(p, ob.U16).encode([f.astype(np.uint16) for f in frame])
     cross, _ = ref.decode(got)
+    cases.assert_irv_matches_reference(out, ref_planes, "cfg5")
     for c in range(3):
         m_ref, p_ref = cases.mse_pae(ref_planes[c], frame[c])
         for planes in (out, cross):

@@ -124,6 +124,7 @@ def _run_case(seed, emu_lib, ref):
         # coefficient on a rounding boundary may flip one quantised value -> the stream length may differ by bytes
         assert abs(len(got) - len(want)) <= max(4, len(want) // 1000), kw
         cross, _ = ref.decode(got)
+        cases.assert_irv_matches_reference(out, ref_planes, kw, list(p.bit_depth))
         for c in range(p.num_comps):
             m_ref, p_ref = cases.mse_pae(ref_planes[c], frame[c])
             for planes in (out, cross):
