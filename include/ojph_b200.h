@@ -185,6 +185,28 @@ int ojb_enc_read_band(ojb_encoder* e, uint32_t tile, uint32_t comp, uint32_t res
 int ojb_enc_band_info(ojb_encoder* e, uint32_t tile, uint32_t comp, uint32_t res, uint32_t band,
                       uint32_t* info8, float* delta2);
 
+/* ---- encode to a target codestream size ---------------------------------------------------
+ * With a target of `bytes` (0 = off, the default), every frame call of the encoder returns a codestream of at
+ * most `bytes`: each code-block's cleanup pass sits at the bit-plane a rate-distortion selection on the device
+ * chose (dropping its k lowest magnitude planes, or the whole block), single layer, readable by any HTJ2K decoder.
+ * A target at or above the unconstrained size gives the unconstrained bytes.  After configure.
+ * Errors: 0x000B0038 the target is below ojb_enc_min_size (also from a frame call after a reconfigure raised it);
+ * 0x000B0039 the configuration codes 64-bit coefficients, or has a tile-part without packets (both refused by
+ * ojb_enc_set_target_size, and by a frame call after a reconfigure to such a configuration);
+ * 0x000B003A an internal consistency check: the selection rounds did not end (each round over the target shrinks the
+ * selection, so this does not happen). */
+int ojb_enc_set_target_size(ojb_encoder* e, uint64_t bytes);
+/* the smallest codestream of the configured geometry: every code-block left out */
+int ojb_enc_min_size(ojb_encoder* e, uint64_t* bytes);
+/* parity hook: the selection of the last frame with a target.  *num_blocks, *kc (entries per block: 1 + the largest
+ * K_max) always; the arrays when not null: kmax[nb], k[nb] (chosen; k = K_max: left out), R[nb * kc] (cleanup bytes
+ * of block b at k, 0xFFFFFFFF: not codable, 0 past the block's top plane), D[nb * kc] (weighted squared error at k,
+ * k <= K_max); info5 = final body budget B*, selection rounds, header and marker bytes, codestream bytes, slope-key
+ * threshold of the final selection (segments with key >= it are taken);
+ * ms4 = distortion, candidate lengths, selection rounds, final block coding */
+int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_t* kmax, uint8_t* k, uint32_t* R,
+                      double* D, uint64_t* info5, float* ms4);
+
 /* ---- decode: ojph::codestream read side ------------------------------------------------- */
 ojb_decoder* ojb_dec_create(void);
 void ojb_dec_destroy(ojb_decoder* d);

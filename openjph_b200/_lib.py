@@ -105,6 +105,9 @@ SYMBOLS = {
     "ojb_enc_encode_resident": (_I, [_VP, _VP, _U64, C.POINTER(_U64), _I]),
     "ojb_enc_kernel_launches": (_U32, [_VP]),
     "ojb_enc_num_blocks": (_U32, [_VP]),
+    "ojb_enc_set_target_size": (_I, [_VP, _U64]),
+    "ojb_enc_min_size": (_I, [_VP, C.POINTER(_U64)]),
+    "ojb_enc_rate_info": (_I, [_VP, C.POINTER(_U32), C.POINTER(_U32), _VP, _VP, _VP, _VP, C.POINTER(_U64), C.POINTER(C.c_float)]),
     "ojb_enc_timings": (None, [_VP, C.POINTER(C.c_float)]),
     "ojb_dec_timings": (None, [_VP, C.POINTER(C.c_float)]),
     "ojb_enc_read_band": (_I, [_VP, _U32, _U32, _U32, _U32, _VP, C.POINTER(_U32), C.POINTER(_U32)]),

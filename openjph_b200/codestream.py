@@ -117,8 +117,9 @@ class _Base:
 
 
 class Encoder(_Base):
-    def __init__(self, params, sample_type=I32, lib=None, comments=None):
-        """comments: the extra COM segments of write_headers(file, comments, n): bytes (binary) or str (text)"""
+    def __init__(self, params, sample_type=I32, lib=None, comments=None, target_bytes=None):
+        """comments: the extra COM segments of write_headers(file, comments, n): bytes (binary) or str (text);
+        target_bytes: every frame call returns a codestream of at most this many bytes (see set_target_size)"""
         super().__init__(lib)
         self.h = self.L.ojb_enc_create()
         if not self.h:
@@ -136,6 +137,36 @@ class Encoder(_Base):
         self.dims = comp_dims(params)
         cap = sum(w * h for w, h in self.dims) * 4 + (1 << 20)
         self._out = np.empty(cap, np.uint8)
+        if target_bytes:
+            self.set_target_size(target_bytes)
+
+    def set_target_size(self, nbytes):
+        """cap every following codestream at nbytes (0: no target).  Each code-block is coded at the bit-plane a
+        rate-distortion selection on the GPU chooses; a target at or above the unconstrained size changes nothing."""
+        self._check(self.L.ojb_enc_set_target_size(self.h, int(nbytes)))
+
+    @property
+    def min_size(self):
+        """the smallest codestream of this geometry (every code-block left out): the lowest target accepted"""
+        n = C.c_uint64()
+        self._check(self.L.ojb_enc_min_size(self.h, C.byref(n)))
+        return int(n.value)
+
+    def rate_info(self):
+        """the selection of the last frame encoded with a target: K_max, chosen k (k == K_max: left out), R[b, k]
+        (cleanup bytes; 0xFFFFFFFF: not codable), D[b, k] (weighted squared error, k <= K_max), the final body budget,
+        the selection rounds, the header and marker bytes, the stream bytes, the slope-key threshold and the stage
+        times (ms)"""
+        nb, kc = C.c_uint32(), C.c_uint32()
+        self._check(self.L.ojb_enc_rate_info(self.h, C.byref(nb), C.byref(kc), None, None, None, None, None, None))
+        n, m = nb.value, kc.value
+        kmax, k = np.zeros(n, np.uint8), np.zeros(n, np.uint8)
+        R, D = np.zeros((n, m), np.uint32), np.zeros((n, m), np.float64)
+        info, ms = (C.c_uint64 * 5)(), (C.c_float * 4)()
+        self._check(self.L.ojb_enc_rate_info(self.h, C.byref(nb), C.byref(kc), kmax.ctypes.data, k.ctypes.data,
+                                             R.ctypes.data, D.ctypes.data, info, ms))
+        return dict(kmax=kmax, k=k, R=R, D=D, budget=int(info[0]), rounds=int(info[1]), header_bytes=int(info[2]),
+                    total=int(info[3]), threshold=int(info[4]), ms=dict(zip(("distortion", "candidates", "selection", "final_encode"), list(ms))))
 
     def close(self):
         if self.h:

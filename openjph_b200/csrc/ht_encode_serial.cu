@@ -50,6 +50,7 @@ struct MelWriter {
 // is done on the whole 64-bit group: the 0xFF bytes are located with SWAR tests and a zero bit is opened
 // above each of them, lowest first -- no byte loop, and groups without 0xFF (the usual case) take the
 // straight path.  One 8-byte store per group.
+template <bool ST = true>
 __device__ __forceinline__ void ms_flush8(MsWriter& s, uint2* dst) {
   const unsigned long long M = 0x0080808080808080ull;         // bytes 0..6: a 0xFF in byte 7 shortens the NEXT group
   const unsigned long long M7 = 0x0101010101010101ull;
@@ -64,7 +65,7 @@ __device__ __forceinline__ void ms_flush8(MsWriter& s, uint2* dst) {
     --c;
     ff = ((x & 0x7F7F7F7F7F7F7F7Full) + M7) & x & M & (~0ull << pos);
   }
-  dst[s.words >> 1] = make_uint2((uint32_t)x, (uint32_t)(x >> 32));
+  if (ST) dst[s.words >> 1] = make_uint2((uint32_t)x, (uint32_t)(x >> 32));
   s.words += 2;
   s.last_ff = ((uint32_t)(x >> 56) == 0xFFu) ? 1u : 0u;
   // drop c (56..64) bits from the window
@@ -75,13 +76,15 @@ __device__ __forceinline__ void ms_flush8(MsWriter& s, uint2* dst) {
   s.nbits -= c;
 }
 // append up to 64 bits; fewer than 64 bits are pending on entry and on exit
+template <bool ST = true>
 __device__ __forceinline__ void ms_put(MsWriter& s, unsigned long long cwd, uint32_t len, uint2* dst) {
   s.w1 = (cwd >> 1) >> (63u - s.nbits);                     // the part that does not fit the low word
   s.w0 |= cwd << s.nbits; s.nbits += len;
-  while (s.nbits >= 64) ms_flush8(s, dst);
+  while (s.nbits >= 64) ms_flush8<ST>(s, dst);
 }
 
 // emit four VLC bytes (needs nbits >= 32); `end` = one past the slot, words grow downward
+template <bool ST = true>
 __device__ __forceinline__ void vlc_flush4(VlcWriter& v, uint32_t* end) {
   const uint32_t lo = (uint32_t)v.acc;
   const uint32_t pv = (lo << 8) | v.prev;
@@ -101,12 +104,13 @@ __device__ __forceinline__ void vlc_flush4(VlcWriter& v, uint32_t* end) {
   }
   v.prev = w >> 24;
   ++v.words;
-  end[-(int)v.words] = __byte_perm(w, 0, 0x0123);
+  if (ST) end[-(int)v.words] = __byte_perm(w, 0, 0x0123);
   v.acc >>= used; v.nbits -= used;
 }
+template <bool ST = true>
 __device__ __forceinline__ void vlc_put(VlcWriter& v, uint32_t cwd, uint32_t len, uint32_t* end) {
   v.acc |= (unsigned long long)cwd << v.nbits; v.nbits += len;
-  while (v.nbits >= 32) vlc_flush4(v, end);
+  while (v.nbits >= 32) vlc_flush4<ST>(v, end);
 }
 
 template <int MS = ES_THREADS>
@@ -131,8 +135,9 @@ __device__ __forceinline__ void mel_event(MelWriter& m, bool one, uint8_t* buf) 
 }
 
 // terminate_mel_vlc :413-441, ms_terminate :517-533: the pending bits of the three streams, the MEL / VLC byte
-// fusion, MEL bytes moved behind MagSgn, Scup
-template <int MS = ES_THREADS>
+// fusion, MEL bytes moved behind MagSgn, Scup.  ST = false: lengths only (nothing is stored; a block the final
+// encode would refuse gets the length RC_LEN_INVALID instead of a status bit)
+template <int MS = ES_THREADS, bool ST = true>
 __device__ __forceinline__ void terminate_block(MsWriter& ms, VlcWriter& vlc, MelWriter& mel, uint8_t* mel_buf, uint8_t* slot,
                                                 uint32_t slot_cap, uint32_t* status, EncResult& res)
 {
@@ -145,13 +150,14 @@ __device__ __forceinline__ void terminate_block(MsWriter& ms, VlcWriter& vlc, Me
       const uint32_t n = lf ? 7u : 8u;
       if (nb < n) break;
       const uint32_t b = (uint32_t)acc & ((1u << n) - 1u);
-      slot[ms_pos++] = (uint8_t)b; acc >>= n; nb -= n; lf = (b == 0xFF);
+      if (ST) slot[ms_pos] = (uint8_t)b;
+      ++ms_pos; acc >>= n; nb -= n; lf = (b == 0xFF);
     }
     const uint32_t cap = lf ? 7u : 8u;
     if (nb) {
       const uint32_t t = cap - nb;
       const uint32_t byte = (uint32_t)acc | ((0xFFu & ((1u << t) - 1u)) << nb);
-      if (byte != 0xFF) slot[ms_pos++] = (uint8_t)byte;
+      if (byte != 0xFF) { if (ST) slot[ms_pos] = (uint8_t)byte; ++ms_pos; }
     } else if (cap == 7) ms_pos--;
   }
   if (mel.run > 0) mel_bit<MS>(mel, 1, mel_buf);
@@ -167,7 +173,8 @@ __device__ __forceinline__ void terminate_block(MsWriter& ms, VlcWriter& vlc, Me
       uint32_t b = (uint32_t)acc & 0xFFu, n = 8;
       if (pv > 0x8F && nb >= 7 && (b & 0x7F) == 0x7F) { b = 0x7F; n = 7; }
       if (nb < n) break;
-      vend[-(int)(++vl_pos)] = (uint8_t)b; acc >>= n; nb -= n; pv = b;
+      ++vl_pos; if (ST) vend[-(int)vl_pos] = (uint8_t)b;
+      acc >>= n; nb -= n; pv = b;
     }
     // the unfinished byte: after a byte > 0x8F only 7 bits are available at first (vlc_encode :379-405)
     vl_tmp = (uint32_t)acc & 0xFFu;
@@ -181,14 +188,16 @@ __device__ __forceinline__ void terminate_block(MsWriter& ms, VlcWriter& vlc, Me
     } else {
       if (mel.pos < ES_MEL_BYTES) mel_buf[mel.pos * MS] = (uint8_t)mel_tmp;
       mel.pos++;
-      vend[-(int)(++vl_pos)] = (uint8_t)vl_tmp;
+      ++vl_pos; if (ST) vend[-(int)vl_pos] = (uint8_t)vl_tmp;
     }
   }
   if (mel.pos > 192 || ms_pos + mel.pos + vl_pos + 8 > slot_cap) {
+    if (!ST) { res.len_head = RC_LEN_INVALID; res.len_tail = 0; return; }
     atomicOr(status, mel.pos > 192 ? 2u : 1u);          // the reference errors out on MEL > 192 bytes
     res.len_head = 0; res.len_tail = 0;
     return;
   }
+  if (!ST) { res.len_head = ms_pos + mel.pos; res.len_tail = vl_pos; return; }
   for (uint32_t i = 0; i < mel.pos; ++i) slot[ms_pos + i] = mel_buf[i * MS];
   const uint32_t scup = mel.pos + vl_pos;
   vend[-1] = (uint8_t)(scup >> 4);
@@ -200,12 +209,14 @@ __device__ __forceinline__ void terminate_block(MsWriter& ms, VlcWriter& vlc, Me
 // WIDE: 64-bit sign-magnitude samples (ojph_encode_codeblock64, src/core/coding/ojph_block_encoder.cpp:1026-1523): the same
 // pass with p = 62 - missing_msbs, exponents up to 6 bits, MagSgn fields of up to 43 bits appended one sample at a time,
 // and the 4-bit U-VLC extension for u_q > 32 (uvlc_tbl entries 33.., :236-247) after the two suffixes (:1491-1492)
-template <bool WIDE>
+// COUNT: the candidate lengths of rate control (rate_ctrl.cu).  Thread i codes block i / kc with its k = i % kc lowest
+// magnitude planes dropped (p + k; only k < ncand[block]) and records the length alone in results[i]; nothing is stored
+template <bool WIDE, bool COUNT = false>
 __global__ void __launch_bounds__(ES_THREADS)
 ht_encode_serial_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
                         const uint32_t* __restrict__ coef32, uint8_t* __restrict__ slots,
                         EncResult* __restrict__ results, const uint16_t* __restrict__ tables,
-                        uint32_t* __restrict__ status, uint32_t prev_quads)
+                        uint32_t* __restrict__ status, uint32_t prev_quads, uint32_t kc = 1, const uint8_t* __restrict__ ncand = nullptr)
 {
   __shared__ uint16_t s_vlc[2 * 2048];
   __shared__ uint16_t s_uvlc[36];
@@ -218,13 +229,20 @@ ht_encode_serial_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
 
   const uint32_t bidx = blockIdx.x * ES_THREADS + threadIdx.x;
   if (bidx >= nblocks) return;
-  const EncBlock blk = blocks[bidx];
-  if (blk.flags & ENC_FLAG_FAST) return;                 // coded by ht_encode_fast_kernel
+  EncBlock blk;
+  if (COUNT) {
+    const uint32_t b = bidx / kc, k = bidx - b * kc;
+    if (k >= ncand[b]) return;
+    blk = blocks[b]; blk.p = (uint16_t)(blk.p + k);
+  } else {
+    blk = blocks[bidx];
+    if (blk.flags & ENC_FLAG_FAST) return;               // coded by ht_encode_fast_kernel
+  }
   typedef typename WordOf<WIDE>::W W;
   constexpr uint32_t WB = WIDE ? 64u : 32u, EB = WIDE ? 6u : 5u, EM = (1u << EB) - 1u;     // word bits; bits of a stored exponent
   const uint32_t width = blk.w, height = blk.h, stride = blk.stride, p = blk.p;
   const W* __restrict__ src = reinterpret_cast<const W*>(coef32) + blk.src_off;
-  uint8_t* slot = slots + blk.slot_off;
+  uint8_t* slot = COUNT ? nullptr : slots + blk.slot_off;
   uint2* ms_dst = reinterpret_cast<uint2*>(slot);          // slots are 16-byte aligned
   uint32_t* vl_end = reinterpret_cast<uint32_t*>(slot + blk.slot_cap);
   uint8_t* mel_buf = s_mel + threadIdx.x;
@@ -338,7 +356,7 @@ ht_encode_serial_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
           if (WIDE) {                         // fields of up to 43 bits: one append per sample (ms_encode64, :1477-1484)
             #pragma unroll
             for (int i = 0; i < 4; ++i)
-              ms_put(ms, (unsigned long long)s[i] & ((1ull << m[i]) - 1ull), m[i], ms_dst);
+              ms_put<!COUNT>(ms, (unsigned long long)s[i] & ((1ull << m[i]) - 1ull), m[i], ms_dst);
           } else {
             const unsigned long long A = (unsigned long long)((uint32_t)s[0] & ((1u << m[0]) - 1u)) |
                                          ((unsigned long long)((uint32_t)s[1] & ((1u << m[1]) - 1u)) << m[0]);
@@ -346,8 +364,8 @@ ht_encode_serial_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
                                          ((unsigned long long)((uint32_t)s[3] & ((1u << m[3]) - 1u)) << m[2]);
             // one append per quad while its four fields fit 64 bits (K_max <= 15), else one per column
             const uint32_t la = m[0] + m[1], lb = m[2] + m[3];
-            if (narrow) ms_put(ms, A | (B << la), la + lb, ms_dst);
-            else { ms_put(ms, A, la, ms_dst); ms_put(ms, B, lb, ms_dst); }
+            if (narrow) ms_put<!COUNT>(ms, A | (B << la), la + lb, ms_dst);
+            else { ms_put<!COUNT>(ms, A, la, ms_dst); ms_put<!COUNT>(ms, B, lb, ms_dst); }
           }
         }
         rho_left = rho;
@@ -376,17 +394,20 @@ ht_encode_serial_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
         bits |= (c1 & 7u) << len; len += (c1 >> 3) & 7u;
         bits |= ((c0 >> 6) & 31u) << len; len += (c0 >> 11) & 31u;
         bits |= ((c1 >> 6) & 31u) << len; len += (c1 >> 11) & 31u;
-        vlc_put(vlc, bits, len, vl_end);
-        if (WIDE && (xl0 | xl1)) vlc_put(vlc, x0 | (x1 << xl0), xl0 + xl1, vl_end);
+        vlc_put<!COUNT>(vlc, bits, len, vl_end);
+        if (WIDE && (xl0 | xl1)) vlc_put<!COUNT>(vlc, x0 | (x1 << xl0), xl0 + xl1, vl_end);
       }
     }
     if (ms.words + vlc.words + 24 >= slot_words) { overflow = true; break; }
   }
 
-  if (overflow) { atomicOr(status, 1u); results[bidx].len_head = 0; results[bidx].len_tail = 0; return; }
+  if (overflow) {
+    if (!COUNT) atomicOr(status, 1u);
+    results[bidx].len_head = COUNT ? RC_LEN_INVALID : 0; results[bidx].len_tail = 0; return;
+  }
   if (any_sig == 0 && negzero == 0) { results[bidx].len_head = 0; results[bidx].len_tail = 0; return; }   // block not included
 
-  terminate_block(ms, vlc, mel, mel_buf, slot, blk.slot_cap, status, results[bidx]);
+  terminate_block<ES_THREADS, !COUNT>(ms, vlc, mel, mel_buf, slot, blk.slot_cap, status, results[bidx]);
 }
 
 // ---- fast path -------------------------------------------------------------------------------------------
@@ -799,6 +820,18 @@ void launch_ht_encode_serial(const EncBlock* blocks, uint32_t nblocks, uint32_t 
     OJB_LAUNCH(ht_encode_serial_kernel<false>, grid, block, smem, sg, blocks, nblocks, coef, slots, results, tables, status,
                prev_quads);
   if (forked) { cudaEventRecord(side->join, side->st); cudaStreamWaitEvent(st, side->join, 0); }
+}
+
+void launch_ht_encode_lengths(const EncBlock* blocks, uint32_t nblocks, uint32_t kc, const uint8_t* ncand, uint32_t max_width,
+                              const uint32_t* coef, EncResult* lengths, const uint16_t* tables, cudaStream_t st)
+{
+  const uint32_t n = nblocks * kc;
+  if (n == 0) return;
+  const uint32_t prev_quads = (max_width + 1) / 2 + 2;
+  const size_t smem = (size_t)prev_quads * ES_THREADS * sizeof(uint16_t);
+  cudaFuncSetAttribute(ht_encode_serial_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  OJB_LAUNCH((ht_encode_serial_kernel<false, true>), dim3((n + ES_THREADS - 1) / ES_THREADS), dim3(ES_THREADS), smem, st,
+             blocks, n, coef, nullptr, lengths, tables, nullptr, prev_quads, kc, ncand);
 }
 
 } // namespace ojb

@@ -386,6 +386,51 @@ int ojb_enc_encode_resident(ojb_encoder* e, uint8_t* out, uint64_t out_cap, uint
   });
 }
 uint32_t ojb_enc_kernel_launches(ojb_encoder* e) { return e->enc.last_launches; }
+int ojb_enc_set_target_size(ojb_encoder* e, uint64_t bytes) {
+  return guarded_on(e->device, [&] {
+    if (!e->configured) fail(0x000B0013, "encoder is not configured");
+    e->enc.set_target(bytes);
+  });
+}
+int ojb_enc_min_size(ojb_encoder* e, uint64_t* bytes) {
+  return guarded_on(e->device, [&] {
+    if (!e->configured) fail(0x000B0013, "encoder is not configured");
+    *bytes = e->enc.min_bytes;
+  });
+}
+int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_t* kmax, uint8_t* k, uint32_t* R,
+                      double* D, uint64_t* info5, float* ms4) {
+  return guarded_on(e->device, [&] {
+    Encoder& E = e->enc;
+    if (!e->configured || E.rc_kc == 0) fail(0x000B0013, "no frame has been encoded with a target size");
+    const uint32_t nb = (uint32_t)E.h_blocks.size(), n = E.rc_kc;
+    *num_blocks = nb; *kc = n;
+    const RcTables& t = E.rc;
+    if (kmax) for (uint32_t b = 0; b < nb; ++b) kmax[b] = (uint8_t)(31u - E.h_blocks[b].p);
+    if (k) cuda_check(cudaMemcpy(k, t.chosen, nb, cudaMemcpyDeviceToHost), "rate_info");
+    if (R) {
+      std::vector<EncResult> c((size_t)nb * n); std::vector<uint8_t> nc(nb);
+      cuda_check(cudaMemcpy(c.data(), t.cand, c.size() * sizeof(EncResult), cudaMemcpyDeviceToHost), "rate_info");
+      cuda_check(cudaMemcpy(nc.data(), t.ncand, nb, cudaMemcpyDeviceToHost), "rate_info");
+      for (uint32_t b = 0; b < nb; ++b)
+        for (uint32_t j = 0; j < n; ++j) {
+          const EncResult& r = c[(size_t)b * n + j];
+          R[(size_t)b * n + j] = j >= nc[b] ? 0u : (r.len_head == RC_LEN_INVALID ? RC_LEN_INVALID : r.len_head + r.len_tail);
+        }
+    }
+    if (D) {
+      cuda_check(cudaMemcpy(D, t.dist, (size_t)nb * n * 8, cudaMemcpyDeviceToHost), "rate_info");
+      for (uint32_t b = 0; b < nb; ++b)
+        for (uint32_t j = 32u - E.h_blocks[b].p; j < n; ++j) D[(size_t)b * n + j] = 0.0;     // past K_max: not computed
+    }
+    if (info5) {
+      RcState s; cuda_check(cudaMemcpy(&s, t.state, sizeof(s), cudaMemcpyDeviceToHost), "rate_info");
+      info5[0] = (uint64_t)s.budget; info5[1] = s.rounds; info5[2] = s.total - s.body; info5[3] = s.total;
+      info5[4] = s.thresh == 0xFFFFFFFFu ? (1ull << 32) : s.thresh;
+    }
+    if (ms4) for (int i = 0; i < 4; ++i) ms4[i] = E.rc_ms[i];
+  });
+}
 void ojb_enc_timings(ojb_encoder* e, float* ms8) {
   for (int i = 0; i < 7; ++i) ms8[i] = e->enc.stage_ms[i];
   ms8[7] = (float)e->enc.host_ms;

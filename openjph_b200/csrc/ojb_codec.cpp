@@ -473,6 +473,8 @@ void Encoder::configure(const Params& p, uint32_t sample_type) {
   main_header.clear();
   params.write_main_header(main_header, nullptr, nullptr, 0);
   build_header_plan();
+  min_bytes = min_size_of_geometry();
+  rc_kc = 0;                           // rate-control tables follow the geometry: planned again on first use
   // line-based front end state
   line_cur.assign(params.num_comps(), 0); cur_comp = 0; lines_done = false;
 }
@@ -480,9 +482,10 @@ void Encoder::configure(const Params& p, uint32_t sample_type) {
 // The static side of pkt_headers.cu: packets in stream order, their bands with blocks (segments), blocks in header
 // order (items), groups of 32 items, tile-parts -- everything that depends on the geometry only.
 void Encoder::build_header_plan() {
-  device_headers = false;
+  device_headers = false; rc_sizing = false;
   memset(&hplan, 0, sizeof(hplan));
-  { const char* e = getenv("OJB_HOST_HEADERS"); if (e && *e && *e != '0') return; }
+  // OJB_HOST_HEADERS=1 keeps the host writer; the plan is still built for rate control, which sizes its selections with it
+  const bool host_writer = [] { const char* e = getenv("OJB_HOST_HEADERS"); return e && *e && *e != '0'; }();
   const bool partial = !tile_mask.empty();        // this rank's tile-parts only: no main header, TLM or EOC (ojb_shard.cpp)
   std::vector<HdrSeg> segs; std::vector<HdrPkt> pkts; std::vector<HdrGroup> groups; std::vector<HdrTp> tps; std::vector<uint32_t> item_seg;
   uint64_t nodes = 0, hoff = 0; uint32_t max_cap = 0;
@@ -522,7 +525,7 @@ void Encoder::build_header_plan() {
     }
     for (size_t i = 0; i < tp_first.size(); ++i) {
       const uint32_t end = (i + 1 < tp_first.size()) ? tp_first[i + 1] : (uint32_t)seq.size();
-      if (end == tp_first[i]) return;                 // a tile-part without packets: the host writer handles it
+      if (end == tp_first[i]) return;                 // a tile-part without packets: the host writer handles it (no rate control)
       tpt.push_back(TpTmp{ t, base + tp_first[i], end - tp_first[i], tp_index[i], tp_total });
       pkts[base + tp_first[i]].tp_first = 1;
     }
@@ -570,7 +573,83 @@ void Encoder::build_header_plan() {
   d_fixed.reserve(fixed_blob.size() + 16);
   CK(cudaMemcpy(d_fixed.p, fixed_blob.data(), fixed_blob.size(), cudaMemcpyHostToDevice));
   h_total.reserve(64);
-  device_headers = true;
+  rc_sizing = true;
+  device_headers = !host_writer;
+}
+
+// the codestream with every code-block left out: main header [+ TLM], SOT + SOD per tile-part, empty packets, EOC
+uint64_t Encoder::min_size_of_geometry() const {
+  uint64_t n = main_header.size() + 2;
+  const std::vector<CodedBlock> empty(layout.num_blocks);
+  std::vector<PacketRef> seq; std::vector<uint32_t> tp_first; std::vector<uint8_t> hdr;
+  uint64_t ntp = 0;
+  for (uint32_t t = 0; t < (uint32_t)layout.tiles.size(); ++t) {
+    layout.packet_sequence(t, seq, tp_first);
+    ntp += tp_first.size();
+    for (const PacketRef& pr : seq) {
+      const ResGeom& rg = layout.res_of(pr);
+      hdr.clear(); write_packet_header(rg, rg.precincts[pr.precinct], empty.data(), hdr);
+      n += hdr.size();
+    }
+  }
+  n += 14 * ntp;
+  if (params.need_tlm) n += 6 + 6 * ntp;
+  return n;
+}
+
+void Encoder::set_target(uint64_t bytes) {
+  if (bytes && wide)
+    fail(0x000B0039, "a target size needs the 32-bit coefficient path: this configuration codes 64-bit coefficients");
+  if (bytes && !rc_sizing)
+    fail(0x000B0039, "a target size needs every tile-part to hold a packet: the device header plan that sizes each "
+         "selection cannot describe an empty tile-part");
+  if (bytes && bytes < min_bytes)
+    fail(0x000B0038, "target of %llu bytes is below the smallest codestream of this geometry (%llu bytes)",
+         (unsigned long long)bytes, (unsigned long long)min_bytes);
+  target_bytes = bytes;
+}
+
+// per-block weights W_b = G_b C_c s_c^2 and the device tables of the selection (see RcTables)
+void Encoder::plan_rate_control() {
+  const uint32_t nb = (uint32_t)h_blocks.size();
+  uint32_t kmax = 0;
+  for (const EncBlock& e : h_blocks) kmax = std::max<uint32_t>(kmax, 31u - e.p);
+  const uint32_t kc = kmax + 1;
+  std::vector<double> wgt(nb, 0.0);
+  std::vector<uint8_t> irv(nb, 0);
+  const Params& P = params;
+  const bool ct = P.color_transform();
+  std::vector<std::vector<double>> gains(P.num_comps());
+  for (uint32_t c = 0; c < P.num_comps(); ++c) gains[c] = P.band_energy_gains(c);
+  for (const TileGeom& t : layout.tiles)
+    for (const TileCompGeom& tc : t.comps)
+      for (const ResGeom& rg : tc.res)
+        for (uint32_t b = 0; b < 4; ++b) {
+          const BandGeom& bg = rg.bands[b];
+          if (bg.empty) continue;
+          const uint32_t c = tc.comp;
+          const bool rev = P.reversible(c);
+          const double G = gains[c][P.subband_index(c, rg.res_num, b)];
+          const double C = (ct && c < 3) ? colour_weight(!P.reversible(0), c) : 1.0;
+          const double s = rev ? 1.0 : (double)P.band_delta(c, rg.res_num, b) * std::ldexp(1.0, (int)P.comps[c].bit_depth);
+          for (uint32_t i = 0; i < bg.nbw * bg.nbh; ++i) { wgt[bg.block_base + i] = G * C * s * s; irv[bg.block_base + i] = rev ? 0 : 1; }
+        }
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 63) & ~(size_t)63; return o; };
+  const size_t o_cand = take((size_t)nb * kc * sizeof(EncResult)), o_dist = take((size_t)nb * kc * 8), o_w = take((size_t)nb * 8);
+  const size_t o_irv = take(nb), o_nc = take(nb), o_hk = take((size_t)nb * (kc + 1)), o_key = take((size_t)nb * kc * 4);
+  const size_t o_len = take((size_t)nb * kc * 4), o_hn = take(nb), o_ch = take(nb), o_st = take(sizeof(RcState));
+  d_rc.reserve(off);
+  uint8_t* base = d_rc.as<uint8_t>();
+  rc.kc = kc;
+  rc.cand = (EncResult*)(base + o_cand); rc.dist = (double*)(base + o_dist); rc.weight = (const double*)(base + o_w);
+  rc.irv = base + o_irv; rc.ncand = base + o_nc; rc.hull_k = base + o_hk; rc.hull_key = (uint32_t*)(base + o_key);
+  rc.hull_len = (uint32_t*)(base + o_len); rc.hull_n = base + o_hn; rc.chosen = base + o_ch; rc.state = (RcState*)(base + o_st);
+  CK(cudaMemcpy(base + o_w, wgt.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(base + o_irv, irv.data(), nb, cudaMemcpyHostToDevice));
+  d_work.reserve(std::max<size_t>(1, nb) * sizeof(EncBlock));
+  h_rc.reserve(64 + nb);
+  rc_kc = kc;
 }
 
 int32_t* Encoder::exchange(const int32_t* line_written, uint32_t& next_comp) {
@@ -624,6 +703,75 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   }
   mark(1);
   uint32_t nb = (uint32_t)h_blocks.size();
+  const bool rc_frame = rc_on() && phase == PHASE_ALL && nb > 0;
+  if (rc_frame) {
+    if (wide) fail(0x000B0039, "a target size needs the 32-bit coefficient path: this configuration codes 64-bit coefficients");
+    if (target_bytes < min_bytes)
+      fail(0x000B0038, "target of %llu bytes is below the smallest codestream of this geometry (%llu bytes)",
+           (unsigned long long)target_bytes, (unsigned long long)min_bytes);
+    if (!rc_sizing)
+      fail(0x000B0039, "a target size needs every tile-part to hold a packet: the device header plan that sizes each "
+           "selection cannot describe an empty tile-part");
+    if (rc_kc == 0) plan_rate_control();
+  }
+  // rate control: the candidates and the rounds of the selection (rate_ctrl.cu); each round sizes its selection with the
+  // packet header kernels, so the block coder's final pass and the headers see the chosen planes in d_work
+  EncBlock* const work = d_work.as<EncBlock>();
+  const EncBlock* const code_blocks = rc_frame ? work : d_blocks.as<EncBlock>();
+  auto rc_size = [&](bool first) {
+    launch_packet_header_total(hplan, work, d_results.as<EncResult>(), 30u, fixed_blob.size(), true, stream);
+    launch_rc_check(rc, hplan.total, target_bytes, min_bytes, first, stream);
+    last_launches += packet_header_total_launches(hplan) + 1;
+  };
+  auto rc_state_out = [&] {
+    launch_ctrl_copy(h_rc.p, rc.state, sizeof(RcState), stream);
+    launch_ctrl_copy(h_rc.as<uint8_t>() + 64, rc.chosen, nb, stream);
+    last_launches += 2;
+  };
+  auto enqueue_rc = [&] {
+    CK(cudaMemsetAsync(rc.state, 0, sizeof(RcState), stream));
+    launch_rc_prepare(d_blocks.as<EncBlock>(), nb, d_coef.as<uint32_t>(), rc, stream);
+    mark(8);
+    launch_ht_encode_lengths(d_blocks.as<EncBlock>(), nb, rc.kc, rc.ncand, max_block_w, d_coef.as<uint32_t>(), rc.cand,
+                             d_tables_enc.as<uint16_t>(), stream);
+    mark(9);
+    launch_rc_hull(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
+    last_launches += 4;
+    rc_size(true);
+    for (int r = 0; r < RC_ROUNDS; ++r) {
+      launch_rc_round(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
+      last_launches += 2;
+      rc_size(false);
+    }
+    rc_state_out();
+    mark(10);
+  };
+  // after the frame's rounds: the rare selection that still does not fit goes on eagerly; true = it changed
+  auto rc_settle = [&]() -> bool {
+    if (!rc_frame || h_rc.as<RcState>()->done) return false;
+    for (int i = 0; !h_rc.as<RcState>()->done; ++i) {
+      // every round over the target strictly lowers the selected body (rc_check_kernel), so there are at most as many
+      // rounds as distinct selections: one more hull segment per block and round at the very worst
+      if ((uint64_t)i > (uint64_t)nb * rc.kc + 2)
+        fail(0x000B003A, "rate control did not settle on a selection that fits the target (internal error)");
+      launch_rc_round(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
+      last_launches += 2;
+      rc_size(false);
+      rc_state_out();
+      CK(cudaStreamSynchronize(stream));
+    }
+    return true;
+  };
+  const bool thread_per_block = (serial_block_encoder() && !few_blocks_warp) || max_block_w > 64 || wide;
+  auto enqueue_code = [&] {
+    if (thread_per_block)
+      launch_ht_encode_serial(code_blocks, nb, num_fast_blocks, max_block_w, d_coef.as<uint32_t>(), d_slots.as<uint8_t>(),
+                              d_results.as<EncResult>(), d_tables_enc.as<uint16_t>(), d_status.as<uint32_t>(), stream, wide, &side);
+    else
+      launch_ht_encode(code_blocks, nb, d_coef.as<uint32_t>(), d_slots.as<uint8_t>(),
+                       d_results.as<EncResult>(), d_tables_enc.as<uint16_t>(), d_status.as<uint32_t>(), stream);
+    last_launches += thread_per_block ? (num_fast_blocks ? 1 : 0) + (num_fast_blocks < nb ? 1 : 0) : 1;
+  };
   // 2. transform + block coding (row regions, ojb_shard.cpp: PHASE_FRONT stops after it -- lengths and bytes of this
   // rank's blocks then travel to the writer --, PHASE_BACK on the writer starts behind it)
   auto enqueue_front = [&] {
@@ -641,15 +789,14 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     }
   mark(2);
   if (phase == PHASE_BACK) { mark(3); return; }
-  const bool thread_per_block = (serial_block_encoder() && !few_blocks_warp) || max_block_w > 64 || wide;
-  if (thread_per_block)
-    launch_ht_encode_serial(d_blocks.as<EncBlock>(), nb, num_fast_blocks, max_block_w, d_coef.as<uint32_t>(), d_slots.as<uint8_t>(),
-                            d_results.as<EncResult>(), d_tables_enc.as<uint16_t>(), d_status.as<uint32_t>(), stream, wide, &side);
-  else
-    launch_ht_encode(d_blocks.as<EncBlock>(), nb, d_coef.as<uint32_t>(), d_slots.as<uint8_t>(),
-                     d_results.as<EncResult>(), d_tables_enc.as<uint16_t>(), d_status.as<uint32_t>(), stream);
-  last_launches += thread_per_block ? (num_fast_blocks ? 1 : 0) + (num_fast_blocks < nb ? 1 : 0) : 1;
+  if (rc_frame) enqueue_rc();
+  enqueue_code();
   mark(3);
+  };
+  auto rc_times = [&] {
+    if (!rc_frame) return;
+    cudaEventElapsedTime(&rc_ms[0], ev[2], ev[8]); cudaEventElapsedTime(&rc_ms[1], ev[8], ev[9]);
+    cudaEventElapsedTime(&rc_ms[2], ev[9], ev[10]); cudaEventElapsedTime(&rc_ms[3], ev[10], ev[3]);
   };
   if (phase == PHASE_FRONT) {
     enqueue_front();
@@ -674,12 +821,14 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
       dev_out = d_out.as<uint8_t>(); cap = std::min<uint64_t>(out_cap, d_out.cap);
     }
     uint64_t total = 0;
-    for (int attempt = 0; attempt < 2; ++attempt) {
+    bool grown = false, recode = false;
+    for (int attempt = 0; ; ++attempt) {
       auto enqueue_all = [&] {
       if (attempt == 0) { enqueue_front(); launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches; mark(4); mark(5); }
+      else if (recode) { enqueue_code(); launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches; }
       if (fixed_blob.size() <= cap) CK(cudaMemcpyAsync(dev_out, d_fixed.p, fixed_blob.size(), cudaMemcpyDeviceToDevice, stream));
       CK(cudaMemsetAsync(hplan.hscr, 0, hscr_bytes, stream));
-      launch_packet_headers(hplan, d_blocks.as<EncBlock>(), d_results.as<EncResult>(), wide ? 62u : 30u, fixed_blob.size(), cap,
+      launch_packet_headers(hplan, code_blocks, d_results.as<EncResult>(), wide ? 62u : 30u, fixed_blob.size(), cap,
                             tile_mask.empty(), dev_out, d_dst.as<uint64_t>(), stream);
       if (!tile_mask.empty() && hplan.ntps) { launch_ctrl_copy(h_tpout.p, hplan.tp_out, (size_t)hplan.ntps * 16, stream); ++last_launches; }
       launch_gather_blocks(d_blocks.as<EncBlock>(), d_results.as<EncResult>(), d_dst.as<uint64_t>(), nb, d_slots.as<uint8_t>(), dev_out, stream);
@@ -689,19 +838,23 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
       };
       // resident form (frame already in HBM, codestream stays there): nothing in the call depends on host data, so
       // the whole thing replays as a graph
-      if (planes == nullptr && out_on_device && phase == PHASE_ALL)
-        run_frame({ (uint64_t)(size_t)dev_out, cap, (uint64_t)nb, (uint64_t)num_fast_blocks, (uint64_t)(size_t)d_slots.p, (uint64_t)(size_t)d_coef.p }, enqueue_all);
+      if (attempt == 0 && planes == nullptr && out_on_device && phase == PHASE_ALL)
+        run_frame({ (uint64_t)(size_t)dev_out, cap, (uint64_t)nb, (uint64_t)num_fast_blocks, (uint64_t)(size_t)d_slots.p, (uint64_t)(size_t)d_coef.p,
+                    rc_frame ? target_bytes : 0, (uint64_t)(size_t)d_rc.p, (uint64_t)(size_t)d_work.p }, enqueue_all);
       else enqueue_all();
       CK(cudaStreamSynchronize(stream));
       CK(cudaGetLastError());
       status_flags = h_status.as<uint32_t>()[0];
       if (status_flags & 2u) fail(0x00020001, "mel encoder's buffer is full");
       if (status_flags & 1u) fail(0x00020005, "block encoder's output slot is full");
+      if (attempt == 0 && rc_settle()) { recode = true; continue; }     // code and lay out the settled selection
+      recode = false;
       total = h_total.as<uint64_t>()[0];
       if (h_total.as<uint64_t>()[1] == 0) break;
       // did not fit: the caller's buffer is too small, or (host output) the staging buffer has to grow once
-      if (total > out_cap || out_on_device || attempt == 1)
+      if (total > out_cap || out_on_device || grown)
         fail(0x000B0030, "output buffer too small: need %zu bytes, have %zu", (size_t)total, out_cap);
+      grown = true;
       d_out.reserve(total + 64); dev_out = d_out.as<uint8_t>(); cap = std::min<uint64_t>(out_cap, d_out.cap);
     }
     host_ms = 0;
@@ -713,6 +866,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     mark(7);
     CK(cudaStreamSynchronize(stream));
     collect(8);
+    rc_times();
     CK(cudaGetLastError());
     std::fill(line_cur.begin(), line_cur.end(), 0u); cur_comp = 0; lines_done = false;
     return (size_t)total;
@@ -728,15 +882,22 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   status_flags = h_status.as<uint32_t>()[0];
   if (status_flags & 2u) fail(0x00020001, "mel encoder's buffer is full");
   if (status_flags & 1u) fail(0x00020005, "block encoder's output slot is full");
+  if (rc_settle()) {
+    enqueue_code();
+    launch_ctrl_copy(h_results.p, d_results.p, (size_t)nb * sizeof(EncResult), stream); ++last_launches;
+    CK(cudaStreamSynchronize(stream));
+    CK(cudaGetLastError());
+  }
 
-  // 3. packet headers and final layout on the host
+  // 3. packet headers and final layout on the host (with a target: at the planes the selection chose)
   const EncResult* res = h_results.as<EncResult>();
+  const uint8_t* chosen = rc_frame ? h_rc.as<uint8_t>() + 64 : nullptr;
   for (uint32_t b = 0; b < nb; ++b) {
     CodedBlock& cb = coded[b];
     uint32_t len = res[b].len_head + res[b].len_tail;
     cb.pass_len[0] = len; cb.pass_len[1] = 0;
     cb.num_passes = len ? 1 : 0;
-    cb.missing_msbs = len ? (uint8_t)((wide ? 62u : 30u) - h_blocks[b].p) : 0;
+    cb.missing_msbs = len ? (uint8_t)((wide ? 62u : 30u) - h_blocks[b].p - (chosen ? chosen[b] : 0u)) : 0;
   }
   struct Pkt { PacketRef ref; std::vector<uint8_t> hdr; uint32_t hdr_len, body; };
   struct TilePart { uint32_t tile, first, count, tp_idx, tp_cnt; uint64_t bytes; };
@@ -863,7 +1024,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   launch_ctrl_copy(d_pieces.p, h_pieces.p, pieces.size() * sizeof(CopyPiece), stream);
   if (nb) launch_ctrl_copy(d_dst.p, h_dst.p, (size_t)nb * 8, stream);
   last_launches += (blob.size() ? 1 : 0) + (pieces.empty() ? 0 : 1) + (nb ? 1 : 0);
-  launch_gather_blocks(d_blocks.as<EncBlock>(), d_results.as<EncResult>(), d_dst.as<uint64_t>(), nb,
+  launch_gather_blocks(code_blocks, d_results.as<EncResult>(), d_dst.as<uint64_t>(), nb,
                        d_slots.as<uint8_t>(), dev_out, stream);
   launch_assemble(d_pieces.as<CopyPiece>(), (uint32_t)pieces.size(), max_piece, d_slots.as<uint8_t>(), d_hdr.as<uint8_t>(), dev_out, stream);
   last_launches += 2;
@@ -872,6 +1033,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   mark(7);
   CK(cudaStreamSynchronize(stream));
   collect(8);
+  rc_times();
   CK(cudaGetLastError());
   // reset the line front end for the next frame
   std::fill(line_cur.begin(), line_cur.end(), 0u); cur_comp = 0; lines_done = false;

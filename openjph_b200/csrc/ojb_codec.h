@@ -153,6 +153,22 @@ public:
   size_t hscr_bytes = 0;
   void build_header_plan();
   size_t out_cap_dev = 0;
+  // rate control (rate_ctrl.cu): with a target, every frame call returns a codestream of at most target_bytes, each
+  // code-block coded at the bit-plane a rate-distortion selection on the device chose.  0 = off.  The selection works
+  // on a per-frame copy of the block array (d_work); the header plan sizes each selection (rc_sizing: it exists)
+  uint64_t target_bytes = 0;
+  uint64_t min_bytes = 0;              // every block left out: depends on the geometry only
+  bool rc_sizing = false;
+  enum { RC_ROUNDS = 3 };              // selection rounds inside the frame's graph; more run eagerly when needed
+  RcTables rc;
+  DeviceBuf d_rc, d_work;
+  PinnedBuf h_rc;                      // RcState, then the chosen k per block
+  uint32_t rc_kc = 0;
+  float rc_ms[4] = {0, 0, 0, 0};       // last frame: distortion, candidate lengths, selection, final encode
+  void set_target(uint64_t bytes);
+  uint64_t min_size_of_geometry() const;
+  void plan_rate_control();
+  bool rc_on() const { return target_bytes != 0; }
 };
 
 struct FrameInfo {

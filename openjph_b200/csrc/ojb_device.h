@@ -65,6 +65,36 @@ inline bool enc_block_is_fast(const EncBlock& e) {
 // both 0 for a block with no significant sample (not included in the packet).
 struct EncResult { uint32_t len_head, len_tail; };
 
+// ---- rate control (rate_ctrl.cu) --------------------------------------------------------
+// a candidate length the final encode would refuse (MEL over 192 bytes, slot overflow): never selected
+#define RC_LEN_INVALID 0xFFFFFFFFu
+// what the rounds that settle the body budget share on the device (one per encoder)
+struct RcState {
+  long long budget;          // body budget B_r of the current round
+  unsigned long long total;  // codestream bytes of the last selection sized
+  unsigned long long sum0;   // sum of R_b(0): the body of the unconstrained stream
+  unsigned long long body;   // sum of the selected R_b(k_b)
+  uint32_t thresh;           // slope key threshold of the last selection
+  uint32_t done;             // the last selection sized fits the target
+  uint32_t rounds;           // selections made (0: the unconstrained stream fits)
+  uint32_t pad;
+};
+// the per-block tables of one frame; kc = 1 + the largest K_max: block b's entries are [b * kc, b * kc + K_max_b]
+struct RcTables {
+  uint32_t kc;
+  uint8_t* ncand;            // candidates k < ncand[b] can be non-empty (the block's top magnitude plane; 1 for ENC_CHECK_NEGZERO)
+  EncResult* cand;           // R_b(k) = len_head + len_tail (RC_LEN_INVALID: not a candidate)
+  double* dist;              // D_b(k), k = 0 .. K_max_b
+  const double* weight;      // W_b
+  const uint8_t* irv;        // 1: irreversible band (h_0 = 1/2)
+  uint8_t* hull_k;           // [b * (kc + 1) + j]: k of hull point j (point 0: excluded, k = K_max)
+  uint32_t* hull_key;        // [b * kc + j]: ordered key of segment j (point j -> j + 1), non-increasing in j
+  uint32_t* hull_len;        // [b * kc + j]: R at hull point j + 1
+  uint8_t* hull_n;           // segments per block
+  uint8_t* chosen;           // chosen k per block
+  RcState* state;
+};
+
 // ---- HT block decoder -------------------------------------------------------------------
 struct DecBlock {
   uint64_t data_off;    // byte offset of the coded bytes in the codestream buffer

@@ -80,6 +80,19 @@ void launch_raster_pack(void* dst, const void* image, const RasterPlanes& pl, ui
 void launch_packet_headers(const HdrPlanDev& plan, const EncBlock* blocks, const EncResult* results, uint32_t mmsb_base,
                            uint64_t fixed_len, uint64_t cap, bool write_eoc, uint8_t* out, uint64_t* dst, cudaStream_t st);
 uint32_t packet_header_launches(const HdrPlanDev& plan);
+// the codestream length alone (plan.total[0]): the sizing step of rate control
+void launch_packet_header_total(const HdrPlanDev& plan, const EncBlock* blocks, const EncResult* results, uint32_t mmsb_base,
+                                uint64_t fixed_len, bool write_eoc, cudaStream_t st);
+uint32_t packet_header_total_launches(const HdrPlanDev& plan);
+
+// rate control (rate_ctrl.cu, and the count-only encoder of ht_encode_serial.cu)
+void launch_ht_encode_lengths(const EncBlock* blocks, uint32_t nblocks, uint32_t kc, const uint8_t* ncand, uint32_t max_width,
+                              const uint32_t* coef, EncResult* lengths, const uint16_t* tables, cudaStream_t st);
+void launch_rc_prepare(const EncBlock* blocks, uint32_t nblocks, const uint32_t* coef, const RcTables& t, cudaStream_t st);
+void launch_rc_hull(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res, const RcTables& t, cudaStream_t st);
+void launch_rc_round(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res, const RcTables& t, cudaStream_t st);
+void launch_rc_check(const RcTables& t, const uint64_t* total, uint64_t target, uint64_t min_bytes, bool first, cudaStream_t st);
+double colour_weight(bool ict, uint32_t c);
 // block pieces computed on the device from per-block results + destination offsets
 void launch_gather_blocks(const EncBlock* blocks, const EncResult* results, const uint64_t* dst_off,
                           uint32_t nblocks, const uint8_t* slots, uint8_t* out, cudaStream_t st);

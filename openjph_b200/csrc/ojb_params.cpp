@@ -359,15 +359,15 @@ void Params::set_precincts(int n, const uint32_t* w, const uint32_t* h) {
   }
 }
 
-// QCD / QCC of a component with a DFS structure and / or an ATK kernel (see KernelGains)
-static void make_part2_steps(QuantSet& q, uint32_t comp, const Params& p) {
+// bands of a component with a DFS structure and / or an ATK kernel in marker order (LL, then for every resolution 1..D
+// the bands its level produces), with their gains measured on the kernel (see KernelGains)
+namespace {
+struct Part2Band { double bibo, norm; uint32_t band; };
+std::vector<Part2Band> part2_bands(uint32_t comp, const Params& p) {
   const AtkSpec& k = p.atk_of(comp);
   const KernelGains g(k);
-  const uint32_t D = q.num_decomps;
-  const bool rev = k.reversible();
-  if (q.qfactor != 0) fail(0x000B0020, "Qfactor needs the 9/7 kernel on a dyadic decomposition");
-  // bands in marker order: LL, then for every resolution 1..D the bands its level produces
-  struct B { double bibo, norm; uint32_t band; };
+  const uint32_t D = p.decomps(comp);
+  typedef Part2Band B;
   std::vector<B> bands;
   auto count = [&](uint32_t upto, bool horz) {          // levels 1..upto that split in this direction
     uint32_t n = 0;
@@ -392,6 +392,16 @@ static void make_part2_steps(QuantSet& q, uint32_t comp, const Params& p) {
       bands.push_back(B{ bx * by, ex * ey, b });
     }
   }
+  return bands;
+}
+} // namespace
+
+// QCD / QCC of a component with a DFS structure and / or an ATK kernel
+static void make_part2_steps(QuantSet& q, uint32_t comp, const Params& p) {
+  const bool rev = p.atk_of(comp).reversible();
+  if (q.qfactor != 0) fail(0x000B0020, "Qfactor needs the 9/7 kernel on a dyadic decomposition");
+  typedef Part2Band B;
+  const std::vector<B> bands = part2_bands(comp, p);
   q.num_subbands = (uint32_t)bands.size();
   if (rev) {
     const uint32_t Bd = q.bit_depth + ((comp < 3 && q.is_color_trans) ? 1u : 0u);
@@ -421,6 +431,24 @@ static void make_part2_steps(QuantSet& q, uint32_t comp, const Params& p) {
     for (size_t i = 0; i < bands.size(); ++i)
       q.SP[i] = pack_step((float)((double)q.base_delta / (bands[i].norm * arr[bands[i].band])));
   }
+}
+
+std::vector<double> Params::band_energy_gains(uint32_t c) const {
+  std::vector<double> g;
+  if (is_part2(c)) {
+    for (const Part2Band& b : part2_bands(c, *this)) g.push_back(b.norm * b.norm);
+    return g;
+  }
+  // the 1-D synthesis gains set_rev_quant / set_irrev_quant weigh the bands with
+  const bool rev = wavelet_of(c) == DWT_REV53;
+  const uint32_t D = decomps(c);
+  const double gl = energy_gain_l(D, rev);
+  g.push_back(gl * gl * gl * gl);
+  for (uint32_t d = D; d > 0; --d) {
+    const double l = energy_gain_l(d, rev), h = energy_gain_h(d - 1, rev);
+    g.push_back(h * l * h * l); g.push_back(l * h * l * h); g.push_back(h * h * h * h);
+  }
+  return g;
 }
 
 static void make_quant_steps(QuantSet& q, uint32_t comp, const Params& p) {

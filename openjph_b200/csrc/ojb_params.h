@@ -175,6 +175,8 @@ struct Params {
   uint32_t subband_index(uint32_t c, uint32_t res, uint32_t band) const;
   uint32_t band_kmax(uint32_t c, uint32_t res, uint32_t band) const { return quant_for(c).kmax_at(subband_index(c, res, band)); }
   float band_delta(uint32_t c, uint32_t res, uint32_t band) const { return quant_for(c).irrev_delta_at(subband_index(c, res, band), band); }
+  // squared L2 norm of one coefficient's synthesis waveform, per sub-band index of component c (rate control's weights)
+  std::vector<double> band_energy_gains(uint32_t c) const;
   uint32_t log_cb_w(uint32_t c) const { const CodStyle* s = find_coc(c); return (s ? s->cb_w_exp : cb_w_exp) + 2u; }
   uint32_t log_cb_h(uint32_t c) const { const CodStyle* s = find_coc(c); return (s ? s->cb_h_exp : cb_h_exp) + 2u; }
   uint32_t log_pp_w(uint32_t c, uint32_t r) const {

@@ -452,6 +452,28 @@ void launch_packet_headers(const HdrPlanDev& pl, const EncBlock* blocks, const E
   }
 }
 
+// the stream size alone: the header kernels up to the layout's prefix sum, with no room to write (pl.total[0] only)
+void launch_packet_header_total(const HdrPlanDev& pl, const EncBlock* blocks, const EncResult* results, uint32_t mmsb_base,
+                                uint64_t fixed_len, bool write_eoc, cudaStream_t st)
+{
+  if (pl.nsegs)
+    OJB_LAUNCH(hdr_trees_kernel, dim3(pl.nsegs), dim3(256), 0, st, pl.segs, blocks, results, mmsb_base, pl.tinc, pl.tmm, pl.tfi, pl.seg_root);
+  if (pl.nitems) {
+    OJB_LAUNCH(hdr_items_kernel, dim3((pl.nitems + 127) / 128), dim3(128), 0, st, pl.segs, pl.pkts, pl.item_seg, pl.nitems, results,
+               pl.tinc, pl.tmm, pl.tfi, pl.seg_root, pl.ibits, pl.inbits, pl.itab, pl.ilen);
+    OJB_LAUNCH(hdr_groups_kernel, dim3((pl.ngroups + HG_GROUPS - 1) / HG_GROUPS), dim3(256), 0, st, pl.groups, pl.ngroups, pl.itab, pl.inbits, pl.ilen,
+               pl.gcomp, pl.gbits, pl.glen);
+  }
+  if (pl.npkts)
+    OJB_LAUNCH(hdr_chain_kernel, dim3(pl.npkts), dim3(HC_THREADS), 0, st, pl.pkts, pl.gcomp, pl.gbits, pl.glen, pl.gstate, pl.gpos, pl.gbody,
+               pl.phdr, pl.pbody);
+  OJB_LAUNCH(hdr_layout_kernel, dim3(1), dim3(HL_THREADS), 0, st, pl.pkts, pl.npkts, pl.tps, pl.ntps, pl.phdr, pl.pbody, fixed_len, (uint64_t)0,
+             write_eoc ? 1u : 0u, pl.ppos, (uint8_t*)nullptr, pl.total, pl.tp_out);
+}
+uint32_t packet_header_total_launches(const HdrPlanDev& pl) {
+  return (pl.nsegs ? 1u : 0u) + (pl.nitems ? 2u : 0u) + (pl.npkts ? 1u : 0u) + 1u;
+}
+
 uint32_t packet_header_launches(const HdrPlanDev& pl) {
   return (pl.nsegs ? 1u : 0u) + (pl.nitems ? 5u : 0u) + (pl.npkts ? 2u : 0u) + 1u;
 }
