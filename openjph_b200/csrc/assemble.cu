@@ -137,8 +137,7 @@ ctrl_copy_kernel(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, siz
 }
 
 __global__ void __launch_bounds__(256)
-dec_merge_kernel(DecBlock* __restrict__ blocks, const DecBlock* __restrict__ proto, const DecDyn* __restrict__ dyn,
-                 const uint64_t* __restrict__ scratch_off, uint32_t n)
+dec_merge_kernel(DecBlock* __restrict__ blocks, const DecBlock* __restrict__ proto, const DecDyn* __restrict__ dyn, uint32_t n)
 {
   const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= n) return;
@@ -147,17 +146,15 @@ dec_merge_kernel(DecBlock* __restrict__ blocks, const DecBlock* __restrict__ pro
   d.data_off = y.data_off; d.len1 = y.len1; d.len2 = y.len2;
   d.num_passes = y.num_passes; d.missing_msbs = y.missing_msbs; d.flags = y.flags;
   if (y.skip) { d.w = 0; d.h = 0; }
-  if (scratch_off) d.scratch_off = scratch_off[b];
   blocks[b] = d;
 }
 
 } // namespace
 
-void launch_dec_merge(DecBlock* blocks, const DecBlock* proto, const DecDyn* dyn, const uint64_t* scratch_off,
-                      uint32_t nblocks, cudaStream_t st)
+void launch_dec_merge(DecBlock* blocks, const DecBlock* proto, const DecDyn* dyn, uint32_t nblocks, cudaStream_t st)
 {
   if (nblocks == 0) return;
-  OJB_LAUNCH(dec_merge_kernel, dim3((nblocks + 255) / 256), dim3(256), 0, st, blocks, proto, dyn, scratch_off, nblocks);
+  OJB_LAUNCH(dec_merge_kernel, dim3((nblocks + 255) / 256), dim3(256), 0, st, blocks, proto, dyn, nblocks);
 }
 
 void launch_ctrl_copy(void* dst, const void* src, size_t bytes, cudaStream_t st)

@@ -1,43 +1,27 @@
 // ht_decode.cu -- HTJ2K block decoder for sm_90a: cleanup pass (+ SigProp + MagRef).
 //
 // Results are those of the reference's ojph_decode_codeblock32
-// (src/core/coding/ojph_block_decoder32.cpp:742-1612).  Two variants, same results:
-//   * ht_decode_serial_kernel (default): the whole cleanup pass by ONE THREAD per code-block, see the
-//     comment above it (lock-step 64-bit refills of 128-bit bit windows);
-//   * step 1 + step 2 (OJB_BLOCK_DECODER=twostep), where the work is split by its dependency structure
-//     rather than by the reference's loop nest:
-//   step 1  MEL + VLC/U-VLC decoding is a strictly serial chain per code-block (each codeword's
-//           position and context depend on the previous one, :869-1089).  A warp cannot speed
-//           one chain up, so ONE THREAD decodes one code-block and a warp runs 32 chains at
-//           once; the per-quad records (rho, e_k, e_1, u) go to a scratch area.
-//   step 2  MagSgn decoding is parallel once bit positions are known: ONE WARP per code-block,
-//           lane i owns quad column i; the MagSgn segment is de-stuffed in parallel into a flat
-//           bit buffer (byte k contributes 7 bits iff byte k-1 is 0xFF), each quad-row does one
-//           warp scan of the per-quad bit counts and every lane extracts its own samples
-//           (:1091-1316).  Exponent prediction needs only the previous quad-row, kept in
-//           registers and exchanged with shuffles.
-//   SPP / MRP  (only present in streams from other encoders) run after step 2.
+// (src/core/coding/ojph_block_decoder32.cpp:742-1612).  One kernel per block class:
+//   * ht_decode_split_kernel: cleanup-only blocks of the common shape (DEC_FLAG_FAST), a producer /
+//     consumer thread pair per code-block, see the comment above it;
+//   * ht_decode_serial_kernel: every other block, the whole cleanup pass by ONE THREAD per code-block
+//     (lock-step 64-bit refills of 128-bit bit windows), then SPP / MRP (only present in streams from
+//     other encoders);
+//   * ht_decode_wide_kernel: 64-bit samples.
 // The de-quantisation the reference does line by line afterwards (tx_from_cb32,
 // src/core/codestream/ojph_codestream_gen.cpp:124-168) is fused into the final store.
 #include "ojb_device.h"
 #include "ojb_kernels.h"
 #include "ojb_async.cuh"
-#include <cstdlib>
 
 namespace ojb {
 
-// minimum CTAs per SM asked of the fast coders (caps registers per thread: 6 -> 85, 7 -> 73, 8 -> 64); more frames'
-// kernels fit on an SM at once, at the price of spills beyond 7
-#ifndef OJB_CODER_MINB
-#define OJB_CODER_MINB 1
-#endif
-#define FULL 0xFFFFFFFFu
 #define DEC_WARPS 4
 
 // block status bits
 #define DST_FAIL 1u
 #define DST_EMPTY 2u              // serial decoder: block not included, to be zero-filled
-#define DEC1_THREADS 128        // step 1: one thread per code-block
+#define DEC1_THREADS 128        // thread-per-block kernels: threads per CTA
 
 namespace {
 
@@ -45,7 +29,7 @@ struct DecTables {            // shared-memory copy
   uint16_t vlc0[1024], vlc1[1024], uvlc0[320], uvlc1[256];
 };
 
-// ---- step 1 readers (thread-private): 32 bits per refill, as the reference's mel_read /
+// ---- MEL / VLC readers (thread-private): 32 bits per refill, as the reference's mel_read /
 // rev_read do (ojph_block_decoder32.cpp:92-152, :307-357), built from aligned word loads
 
 struct MelDec {
@@ -115,7 +99,7 @@ __device__ __forceinline__ int mel_next_run(MelDec& m) {
 
 struct RevDec {               // backward-growing stream (VLC, MRP)
   const uint8_t* p; int size; unsigned long long tmp; uint32_t bits; bool unstuff;
-  // step 1: the stream is read backward one aligned word per refill.  The words are requested
+  // rev_fill32: the stream is read backward one aligned word per refill.  The words are requested
   // VLC_RING-1 refills ahead with cp.async into a per-thread ring in shared memory (global/L2
   // latency is several refill periods for one serial chain per thread); `lo`/`hi` hold the two
   // words the next refill's funnel shift needs.
@@ -144,7 +128,7 @@ __device__ __forceinline__ void rev_prime(RevDec& v, const uint8_t* buffer_start
   for (int i = 0; i < VLC_RING - 1; ++i) rev_ring_issue<STRIDE>(v);
   v.ridx = 0;                                  // oldest request sits in slot 0
 }
-// byte-wise refill (refinement passes, lane 0 only)
+// byte-wise refill (refinement passes)
 __device__ __forceinline__ void rev_fill(RevDec& v) {       // LSB first
   while (v.bits <= 56) {
     uint32_t d = 0;
@@ -198,133 +182,6 @@ __device__ __forceinline__ void rev_fill32(RevDec& v) {
   v.bits += nb;
 }
 
-__global__ void __launch_bounds__(DEC1_THREADS)
-ht_dec_step1_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
-                    const uint8_t* __restrict__ cs, uint32_t* __restrict__ scratch,
-                    const uint16_t* __restrict__ tables, uint32_t* __restrict__ block_status)
-{
-  __shared__ DecTables T;
-  __shared__ uint32_t s_ring[VLC_RING * DEC1_THREADS];     // per-thread FIFO of VLC words (slot-major)
-  {
-    uint16_t* d = reinterpret_cast<uint16_t*>(&T);
-    for (uint32_t i = threadIdx.x; i < sizeof(DecTables) / 2; i += blockDim.x) d[i] = tables[i];
-  }
-  __syncthreads();
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= nblocks) return;
-  const DecBlock blk = blocks[b];
-  uint32_t np = blk.num_passes;
-  if (np == 0 || blk.len1 == 0) { block_status[b] = 0; return; }     // empty block: zero-filled later
-  // validity gates (:752-820)
-  if (np > 1 && blk.len2 == 0) np = 1;
-  bool ok = true;
-  if (np > 3 || blk.missing_msbs >= 30 || blk.len1 < 2) ok = false;
-  if (blk.missing_msbs == 29 && np > 1) np = 1;      // p == 1: refinement passes are skipped
-  const uint8_t* data = cs + blk.data_off;
-  int lcup = (int)blk.len1, scup = 0;
-  if (ok) {
-    scup = ((int)data[lcup - 1] << 4) + (data[lcup - 2] & 0xF);
-    if (scup < 2 || scup > lcup || scup > 4079) ok = false;
-  }
-  if (!ok || blk.w > 64) { block_status[b] = DST_FAIL; return; }
-
-  MelDec mel; mel.p = data + lcup - scup; mel.size = scup - 1; mel.tmp = 0; mel.bits = 0;
-  mel.unstuff = false; mel.k = 0;
-  RevDec vlc; vlc.p = data + lcup - 2; vlc.size = scup - 2;
-  {
-    uint32_t d = *vlc.p--;
-    vlc.tmp = d >> 4;
-    vlc.bits = 4 - (((vlc.tmp & 7) == 7) ? 1u : 0u);
-    vlc.unstuff = (d | 0xF) > 0x8F;
-  }
-  rev_prime(vlc, cs, s_ring + threadIdx.x);
-  mel_prime(mel);
-  int run = mel_next_run(mel);
-
-  const uint32_t width = blk.w, height = blk.h;
-  const uint32_t nq = (width + 1) >> 1, qstride = (nq + 1) & ~1u;   // quads per row (even stride)
-  uint32_t* rec = scratch + blk.scratch_off;
-  uint32_t prev_bl = 0, prev_br = 0;      // bit q: bottom-left / bottom-right significance of the row above
-
-  for (uint32_t y = 0; y < height; y += 2) {
-    const uint16_t* vtab = y ? T.vlc1 : T.vlc0;
-    uint32_t cur_bl = 0, cur_br = 0, rho_left = 0;
-    uint32_t* rrow = rec + (size_t)(y >> 1) * qstride;
-    for (uint32_t q = 0; q < nq; q += 2) {
-      uint32_t t[2] = {0, 0};
-      #pragma unroll
-      for (uint32_t i = 0; i < 2; ++i) {
-        const uint32_t qq = q + i;
-        if (qq < nq) {
-          uint32_t c;
-          if (y == 0) c = (rho_left & 1) | (rho_left >> 1);
-          else {
-            const uint32_t a = (((prev_br << 1) >> qq) | (prev_bl >> qq)) & 1u;
-            const uint32_t l = ((rho_left >> 2) | (rho_left >> 3)) & 1u;
-            const uint32_t r = ((prev_br >> qq) | (qq < 31 ? (prev_bl >> (qq + 1)) : 0u)) & 1u;
-            c = a | (l << 1) | (r << 2);
-          }
-          rev_fill32(vlc);
-          uint32_t e = vtab[(c << 7) | ((uint32_t)vlc.tmp & 0x7F)];
-          if (c == 0) {               // significance of an all-zero context comes from MEL
-            run -= 2;
-            if (run != -1) e = 0;
-            if (run < 0) run = mel_next_run(mel);
-          }
-          vlc.tmp >>= (e & 7); vlc.bits -= (e & 7);
-          t[i] = e;
-          rho_left = (e >> 4) & 15u;
-          cur_bl |= ((rho_left >> 1) & 1u) << qq;
-          cur_br |= ((rho_left >> 3) & 1u) << qq;
-        }
-      }
-      // U-VLC of the pair (:940-974 initial row, :1066-1085 others)
-      uint32_t mode = ((t[0] >> 3) & 1u) | (((t[1] >> 3) & 1u) << 1);
-      uint32_t ent;
-      rev_fill32(vlc);
-      if (y == 0) {
-        if (mode == 3) {
-          run -= 2;
-          if (run == -1) mode = 4;
-          if (run < 0) run = mel_next_run(mel);
-        }
-        ent = T.uvlc0[(mode << 6) | ((uint32_t)vlc.tmp & 0x3F)];
-      } else
-        ent = T.uvlc1[(mode << 6) | ((uint32_t)vlc.tmp & 0x3F)];
-      vlc.tmp >>= (ent & 7); vlc.bits -= (ent & 7);
-      ent >>= 3;
-      uint32_t len = ent & 0xF;
-      uint32_t suf = (uint32_t)vlc.tmp & ((1u << len) - 1u);
-      vlc.tmp >>= len; vlc.bits -= len;
-      ent >>= 4;
-      len = ent & 7; ent >>= 3;
-      const uint32_t kap = (y == 0) ? 1u : 0u;
-      uint32_t u0 = kap + (ent & 7) + (suf & ~(0xFFu << len));
-      uint32_t u1 = kap + (ent >> 3) + (suf >> len);
-      // qstride is even and the scratch offset a multiple of 4 words: one 8-byte store per pair
-      *reinterpret_cast<uint2*>(rrow + q) = make_uint2((t[0] & 0xFFFF) | (u0 << 16), (t[1] & 0xFFFF) | (u1 << 16));
-    }
-    prev_bl = cur_bl; prev_br = cur_br;
-  }
-  block_status[b] = (np << 8);        // ok; effective number of passes for step 2
-}
-
-// ---- step 2 --------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t load_u32_unaligned(const uint8_t* p) {
-  const uint32_t* a = reinterpret_cast<const uint32_t*>((size_t)p & ~(size_t)3);
-  uint32_t sh = (uint32_t)((size_t)p & 3) * 8;
-  uint32_t lo = a[0];
-  if (sh == 0) return lo;
-  return __funnelshift_r(lo, a[1], sh);
-}
-
-// fetch 32 bits at bit position pos from a word buffer of nwords words followed by two words of
-// ones (an exhausted MagSgn stream reads as 0xFF bytes)
-__device__ __forceinline__ uint32_t fetch_bits(const uint32_t* buf, uint32_t pos, uint32_t nwords) {
-  const uint32_t wi = min(pos >> 5, nwords);
-  return __funnelshift_r(buf[wi], buf[wi + 1], pos & 31);
-}
-
 __device__ __forceinline__ uint32_t to_output(uint32_t sm, uint32_t mode, uint32_t shift, float delta) {
   if (mode == DEC_OUT_SIGNMAG) return sm;
   if (mode == DEC_OUT_INT) {
@@ -335,7 +192,7 @@ __device__ __forceinline__ uint32_t to_output(uint32_t sm, uint32_t mode, uint32
   return __float_as_uint(f) | (sm & 0x80000000u);
 }
 
-// simple byte-wise readers for the refinement passes (lane 0 only)
+// simple byte-wise readers for the refinement passes
 struct FwdBits {              // SPP: forward, 0 fed when exhausted, 7-bit byte after 0xFF
   const uint8_t* p; int size; unsigned long long tmp; uint32_t bits; bool unstuff;
 };
@@ -361,7 +218,7 @@ __device__ __forceinline__ uint32_t rec_rho(const uint32_t* rec, uint32_t qstrid
   return ((r >> 4) >> (2 * (x & 1) + (y & 1))) & 1u;
 }
 
-// SigProp + MagRef, serial restatement executed by one lane on the block's sign-magnitude
+// SigProp + MagRef, serial restatement executed by the block's thread on its sign-magnitude
 // samples (ojph_block_decoder32.cpp:1318-1612)
 __device__ void refine_passes(const DecBlock& blk, uint32_t np, const uint8_t* data, uint32_t* dst,
                               const uint32_t* rec, uint32_t qstride, uint32_t p)
@@ -446,207 +303,11 @@ __device__ void refine_passes(const DecBlock& blk, uint32_t np, const uint8_t* d
   }
 }
 
-__global__ void __launch_bounds__(DEC_WARPS * 32)
-ht_dec_step2_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
-                    const uint8_t* __restrict__ cs, uint32_t* __restrict__ coef,
-                    uint32_t* __restrict__ scratch, uint32_t out_mode,
-                    uint32_t* __restrict__ block_status, uint32_t ms_cap_words)
-{
-  __shared__ uint32_t s_stage[DEC_WARPS][40];
-  OJB_DYN_SMEM(uint32_t, s_ms);          // DEC_WARPS x ms_cap_words: de-stuffed MagSgn when it fits
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t b = blockIdx.x * DEC_WARPS + warp;
-  if (b >= nblocks) return;
-  const DecBlock blk = blocks[b];
-  const uint32_t width = blk.w, height = blk.h, stride = blk.stride;
-  uint32_t* dst = coef + blk.dst_off;
-  const uint32_t st = block_status[b];
-  const uint32_t np = st >> 8;
-  const uint32_t shift = 31u - blk.K_max;
-  const float delta = blk.delta;
-  if (out_mode == DEC_OUT_PER_BLOCK) out_mode = (blk.flags & 2) ? (uint32_t)DEC_OUT_FLOAT : (uint32_t)DEC_OUT_INT;
-
-  bool fail = (st & DST_FAIL) != 0;
-  const bool empty = (np == 0) && !fail;
-  const uint32_t nq = (width + 1) >> 1, qstride = (nq + 1) & ~1u;
-  const uint32_t* rec = scratch + blk.scratch_off;
-  const uint32_t nqrows = (height + 1) >> 1;
-  uint32_t* msbuf = scratch + blk.scratch_off + (size_t)qstride * nqrows;   // de-stuffed MagSgn words
-  if ((blk.len1 >> 2) + 4 <= ms_cap_words) msbuf = s_ms + (size_t)warp * ms_cap_words;
-  const uint32_t x = 2 * lane;
-  const bool has0 = x < width, has1 = x + 1 < width;
-  const bool vec2 = ((blk.dst_off | stride) & 1u) == 0;      // block rows 8-byte aligned
-  const uint32_t mmsbp2 = blk.missing_msbs + 2u;
-  const uint32_t p = 30u - blk.missing_msbs;
-
-  if (!fail && !empty) {
-    const uint8_t* data = cs + blk.data_off;
-    const int lcup = (int)blk.len1;
-    const int scup = ((int)data[lcup - 1] << 4) + (data[lcup - 2] & 0xF);
-    const uint32_t mslen = (uint32_t)(lcup - scup);
-    // ---- de-stuff the MagSgn segment: 128 raw bytes per step
-    uint32_t nbits_total = 0;           // bits written so far
-    uint32_t carry_word = 0;            // partial last word (bits nbits_total & 31)
-    bool prev_ff = false;
-    uint32_t* stage = s_stage[warp];
-    uint32_t w_next = (4 * lane < mslen) ? load_u32_unaligned(data + 4 * lane) : 0xFFFFFFFFu;
-    for (uint32_t base = 0; base < mslen; base += 128) {
-      const uint32_t off = base + 4 * lane;
-      uint32_t w = w_next;                  // the next 128 bytes are requested while these are unpacked
-      if (off + 128 < mslen) w_next = load_u32_unaligned(data + off + 128);
-      else w_next = 0xFFFFFFFFu;
-      if (off < mslen && off + 4 > mslen) w |= 0xFFFFFFFFu << (8 * (mslen - off));    // beyond the segment: 0xFF
-      const uint32_t lastb = w >> 24;
-      uint32_t pv = __shfl_up_sync(FULL, lastb, 1);
-      const bool pff = lane ? (pv == 0xFF) : prev_ff;
-      // common case: a full chunk without any 0xFF byte ahead of another byte -> every byte carries
-      // 8 bits and the chunk is a plain 1024-bit shift by the carry length
-      {
-        uint32_t ff = w & (w >> 1); ff &= ff >> 2; ff &= ff >> 4;        // bit 8i set <=> byte i == 0xFF
-        if (base + 128 <= mslen && !__any_sync(FULL, pff || (ff & 0x00010101u))) {
-          const uint32_t cb = nbits_total & 31;
-          uint32_t lo = __shfl_up_sync(FULL, w, 1);
-          uint32_t o = lane ? __funnelshift_l(lo, w, cb) : (carry_word | (w << cb));
-          msbuf[(nbits_total >> 5) + lane] = o;
-          const uint32_t w31 = __shfl_sync(FULL, w, 31);
-          carry_word = cb ? (w31 >> (32 - cb)) : 0u;
-          prev_ff = (w31 >> 24) == 0xFF;
-          nbits_total += 1024;
-          continue;
-        }
-      }
-      const uint32_t b0 = w & 0xFF, b1 = (w >> 8) & 0xFF, b2 = (w >> 16) & 0xFF, b3 = w >> 24;
-      const uint32_t n0 = 8 - (pff ? 1u : 0u), n1 = 8 - (b0 == 0xFF ? 1u : 0u),
-                     n2 = 8 - (b1 == 0xFF ? 1u : 0u), n3 = 8 - (b2 == 0xFF ? 1u : 0u);
-      uint32_t t = b0 & ((1u << n0) - 1u);
-      t |= (b1 & ((1u << n1) - 1u)) << n0;
-      t |= (b2 & ((1u << n2) - 1u)) << (n0 + n1);
-      t |= (b3 & ((1u << n3) - 1u)) << (n0 + n1 + n2);
-      uint32_t n = (off < mslen) ? (n0 + n1 + n2 + n3) : 0u;
-      if (off < mslen && off + 4 > mslen) {           // partial last word: count only real bytes
-        const uint32_t k = mslen - off;
-        n = n0 + (k > 1 ? n1 : 0) + (k > 2 ? n2 : 0);
-        t &= (n < 32) ? ((1u << n) - 1u) : 0xFFFFFFFFu;
-      }
-      uint32_t incl = n;
-      #pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { uint32_t o = __shfl_up_sync(FULL, incl, d); if ((int)lane >= d) incl += o; }
-      const uint32_t tot = __shfl_sync(FULL, incl, 31);
-      const uint32_t cb = nbits_total & 31;
-      // stage: carry bits then this chunk's bits
-      for (uint32_t i = lane; i < 36; i += 32) stage[i] = 0;
-      __syncwarp();
-      if (lane == 0) stage[0] = carry_word;
-      __syncwarp();
-      if (n) {
-        const uint32_t o = cb + incl - n;
-        const unsigned long long v = (unsigned long long)t << (o & 31);
-        atomicOr(&stage[o >> 5], (uint32_t)v);
-        if ((uint32_t)(v >> 32)) atomicOr(&stage[(o >> 5) + 1], (uint32_t)(v >> 32));
-      }
-      __syncwarp();
-      const uint32_t nb = cb + tot, nw = nb >> 5;
-      uint32_t* o32 = msbuf + (nbits_total >> 5);
-      for (uint32_t i = lane; i < nw; i += 32) o32[i] = stage[i];
-      carry_word = stage[nw];
-      __syncwarp();
-      nbits_total += tot;
-      // last real byte of this chunk decides the stuffing of the next chunk's first byte
-      const uint32_t last_off = min(mslen, base + 128) - 1 - base;     // byte index within the chunk
-      const uint32_t wsrc = __shfl_sync(FULL, w, last_off >> 2);
-      prev_ff = ((wsrc >> (8 * (last_off & 3))) & 0xFF) == 0xFF;
-    }
-    // tail: remaining bits + ones (an exhausted MagSgn stream reads as 0xFF bytes)
-    const uint32_t ms_words = (nbits_total >> 5) + 1;
-    if (lane == 0) msbuf[nbits_total >> 5] = carry_word | ((nbits_total & 31) ? (0xFFFFFFFFu << (nbits_total & 31)) : 0xFFFFFFFFu);
-    if (lane < 2) msbuf[ms_words + lane] = 0xFFFFFFFFu;
-    __syncwarp();
-
-    // ---- quad rows
-    uint32_t pos = 0;                       // MagSgn bit position
-    uint32_t pv1 = 0, pv3 = 0;              // v_n of bottom-left / bottom-right sample of the row above
-    uint32_t r_next = (lane < nq) ? rec[lane] : 0;
-    for (uint32_t y = 0; y < height; y += 2) {
-      const uint32_t r = r_next;            // the next row's records are requested a row ahead
-      if (y + 2 < height) r_next = (lane < nq) ? rec[(size_t)((y >> 1) + 1) * qstride + lane] : 0;
-      const uint32_t inf = r & 0xFFFF, uq = r >> 16;
-      const uint32_t rho = (inf >> 4) & 15u;
-      uint32_t Uq;
-      if (y == 0) Uq = uq;
-      else {
-        uint32_t l = __shfl_up_sync(FULL, pv3, 1); if (lane == 0) l = 0;
-        uint32_t rr = __shfl_down_sync(FULL, pv1, 1); if (lane == 31) rr = 0;
-        const uint32_t emax = 31u - (uint32_t)__clz((int)((l | pv1 | pv3 | rr) | 2u));
-        const uint32_t kappa = (rho & (rho - 1)) ? emax : 1u;
-        Uq = uq + kappa;
-      }
-      if (__any_sync(FULL, (lane < nq) && Uq > mmsbp2)) { fail = true; break; }
-      const uint32_t ek = inf >> 12, e1 = (inf >> 8) & 15u;
-      uint32_t m[4];
-      #pragma unroll
-      for (int i = 0; i < 4; ++i) m[i] = ((rho >> i) & 1u) ? Uq - ((ek >> i) & 1u) : 0u;
-      const uint32_t mine = (lane < nq) ? (m[0] + m[1] + m[2] + m[3]) : 0u;
-      uint32_t incl = mine;
-      #pragma unroll
-      for (int d = 1; d < 32; d <<= 1) { uint32_t o = __shfl_up_sync(FULL, incl, d); if ((int)lane >= d) incl += o; }
-      const uint32_t tot = __shfl_sync(FULL, incl, 31);
-      const uint32_t bp = pos + incl - mine;
-      uint32_t out[4], vn[4], msw[4];
-      msw[0] = fetch_bits(msbuf, bp, ms_words);                      // four independent fetches
-      msw[1] = fetch_bits(msbuf, bp + m[0], ms_words);
-      msw[2] = fetch_bits(msbuf, bp + m[0] + m[1], ms_words);
-      msw[3] = fetch_bits(msbuf, bp + m[0] + m[1] + m[2], ms_words);
-      #pragma unroll
-      for (int i = 0; i < 4; ++i) {               // branch-free: insignificant samples are selected away
-        const bool sig = (rho >> i) & 1u;
-        const uint32_t ms = msw[i];
-        const uint32_t v = (ms & ((1u << m[i]) - 1u)) | (((e1 >> i) & 1u) << m[i]) | 1u;
-        vn[i] = sig ? v : 0u;
-        out[i] = sig ? ((ms << 31) | ((v + 2u) << (p - 1))) : 0u;
-      }
-      pos += tot;
-      pv1 = vn[1]; pv3 = vn[3];
-      const uint32_t om = (np > 1) ? (uint32_t)DEC_OUT_SIGNMAG : out_mode;
-      uint32_t* r0 = dst + (size_t)y * stride;
-      const uint32_t o0 = to_output(out[0], om, shift, delta), o2 = to_output(out[2], om, shift, delta);
-      if (vec2 && has1) *reinterpret_cast<uint2*>(r0 + x) = make_uint2(o0, o2);      // 8-byte aligned rows
-      else { if (has0) r0[x] = o0; if (has1) r0[x + 1] = o2; }
-      if (y + 1 < height) {
-        uint32_t* r1 = r0 + stride;
-        const uint32_t o1 = to_output(out[1], om, shift, delta), o3 = to_output(out[3], om, shift, delta);
-        if (vec2 && has1) *reinterpret_cast<uint2*>(r1 + x) = make_uint2(o1, o3);
-        else { if (has0) r1[x] = o1; if (has1) r1[x + 1] = o3; }
-      }
-    }
-
-    if (!fail && np > 1) {
-      __syncwarp();
-      __threadfence_block();
-      if (lane == 0) refine_passes(blk, np, data, dst, rec, qstride, p);
-      __syncwarp();
-      __threadfence_block();
-      if (out_mode != DEC_OUT_SIGNMAG)
-        for (uint32_t yy = 0; yy < height; ++yy)
-          for (uint32_t xx = lane; xx < width; xx += 32) {
-            uint32_t* q = dst + (size_t)yy * stride + xx;
-            *q = to_output(*q, out_mode, shift, delta);
-          }
-    }
-  }
-
-  if (fail || empty) {                      // not decodable / not included: a block of zeros
-    for (uint32_t yy = 0; yy < height; ++yy)
-      for (uint32_t xx = lane; xx < width; xx += 32) dst[(size_t)yy * stride + xx] = 0;
-    if (lane == 0) block_status[b] = fail ? DST_FAIL : 0u;
-  } else if (lane == 0) block_status[b] = 0;
-}
-
 // ---- whole cleanup pass, one thread per code-block ---------------------------------------------
-// The serial form of the decoder (what ojph_decode_codeblock32 does, :742-1316, minus its two-step
-// split): the thread that decodes a quad pair's VLC / U-VLC codewords reads the pair's MagSgn bits
-// right away, so no quad records travel through memory and no warp-wide scan or shared bit buffer
-// is needed -- 586 M warp instructions per 8K frame against 960 M for step 1 + step 2.  Blocks that carry SPP / MRP
-// passes still write their quad records (refine_passes needs the CUP significance).
+// The serial form of the decoder (what ojph_decode_codeblock32 does, :742-1316, in one pass instead of
+// its two): the thread that decodes a quad pair's VLC / U-VLC codewords reads the pair's MagSgn bits
+// right away, so no quad records travel through memory.  Blocks that carry SPP / MRP passes still write
+// their quad records to the scratch area (refine_passes needs the CUP significance).
 // ---- bit readers of the thread-per-block decoder ------------------------------------------------
 // Both streams are read as aligned 8-byte groups through per-thread cp.async rings; a group is un-stuffed
 // as a whole (the positions to delete come from one SWAR test, the usual group has none) and appended to a
@@ -802,7 +463,7 @@ ht_decode_serial_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
   const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= nblocks) return;
   const DecBlock blk = blocks[b];
-  if (blk.flags & DEC_FLAG_FAST) return;                 // decoded by ht_decode_fast_kernel
+  if (blk.flags & DEC_FLAG_FAST) return;                 // decoded by ht_decode_split_kernel
   uint32_t np = blk.num_passes;
   if (np == 0 || blk.len1 == 0) { block_status[b] = DST_EMPTY; return; }     // zero-filled by the fill kernel
   // validity gates (:752-820)
@@ -1012,11 +673,11 @@ ht_decode_serial_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
 }
 
 
-// ---- fast path of the thread-per-block decoder ------------------------------------------------------------
-// The same cleanup pass for the blocks the host marks DEC_FLAG_FAST: one coding pass, width a multiple of 4 and
-// at most 64, even height, 16-byte aligned rows, missing_msbs + 2 <= 16 (so the four MagSgn fields of a quad fit
-// 64 bits).  Knowing that at compile time removes the per-quad bounds / pass / width tests of the general kernel,
-// and the state of the row above shrinks to registers plus one word per quad pair:
+// ---- fast path: two threads per code-block ----------------------------------------------------------------------
+// The cleanup pass of the blocks the host marks DEC_FLAG_FAST: one coding pass, width a multiple of 4 and at most 64,
+// even height, 16-byte aligned rows, missing_msbs + 2 <= 16 (so the four MagSgn fields of a quad fit 64 bits).
+// Knowing that at compile time removes the per-quad bounds / pass / width tests of the general kernel, and the state
+// of the row above shrinks to registers plus one word per quad pair:
 //   * significance of the bottom samples of the row above: a 64-bit register, two bits per quad, walked four bits
 //     per pair; the contexts of both quads of a pair come out of six consecutive bits;
 //   * exponent predictor: per quad boundary q the OR g[q] = h(br of quad q-1) | h(bl of quad q) with h = v_n >> 1
@@ -1025,193 +686,12 @@ ht_decode_serial_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
 //   * VLC through a 64-bit window refilled 32 bits at a time (a pair reads at most 30 bits), MagSgn through the
 //     128-bit window in 8-byte groups as in the general kernel.
 // A U_q beyond missing_msbs + 2 (corrupt data) is clamped and flagged; the block is then zero-filled.
-template <int MODE>       // 0: integer output, 1: float output, 2: sign-magnitude (kernel-level parity entry point)
-__global__ void __launch_bounds__(DEC1_THREADS, OJB_CODER_MINB)
-ht_decode_fast_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
-                      const uint8_t* __restrict__ cs, uint32_t* __restrict__ coef,
-                      const uint16_t* __restrict__ tables, uint32_t* __restrict__ block_status)
-{
-#ifdef OJB_DEC_TABLES_GLOBAL
-  const DecTables& T = *reinterpret_cast<const DecTables*>(tables);       // 5 KB, hot in L1
-#else
-  __shared__ DecTables T;
-#endif
-  __shared__ uint32_t s_vring[VLC_RING * DEC1_THREADS];    // per-thread FIFO of VLC words (slot-major)
-  __shared__ uint2 s_mring[VLC_RING * DEC1_THREADS];       // per-thread FIFO of MagSgn 8-byte groups
-  __shared__ uint32_t s_g[17 * DEC1_THREADS];              // g[2j] | g[2j+1] << 16 of the row above, per pair j
-#ifndef OJB_DEC_TABLES_GLOBAL
-  {
-    uint16_t* d = reinterpret_cast<uint16_t*>(&T);
-    for (uint32_t i = threadIdx.x; i < sizeof(DecTables) / 2; i += blockDim.x) d[i] = tables[i];
-  }
-  __syncthreads();
-#endif
-  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= nblocks) return;
-  const DecBlock blk = blocks[b];
-  if (!(blk.flags & DEC_FLAG_FAST)) return;
-  const uint8_t* data = cs + blk.data_off;
-  const int lcup = (int)blk.len1;
-  const int scup = ((int)data[lcup - 1] << 4) + (data[lcup - 2] & 0xF);
-  if (scup < 2 || scup > lcup || scup > 4079) { block_status[b] = DST_FAIL; return; }
-
-  MelDec mel; mel.p = data + lcup - scup; mel.size = scup - 1; mel.tmp = 0; mel.bits = 0;
-  mel.unstuff = false; mel.k = 0;
-  RevDec vlc; vlc.p = data + lcup - 2; vlc.size = scup - 2;
-  {
-    const uint32_t d = *vlc.p--;                            // the byte that shares the Scup nibble (rev_init, :270-302)
-    vlc.tmp = d >> 4;
-    vlc.bits = 4 - (((vlc.tmp & 7) == 7) ? 1u : 0u);
-    vlc.unstuff = (d | 0xF) > 0x8F;
-  }
-  rev_prime(vlc, cs, s_vring + threadIdx.x);
-  mel_prime(mel);
-  MsDec ms;
-  ms_prime(ms, data, lcup - scup, data + lcup, s_mring + threadIdx.x);
-  int run = mel_next_run(mel);
-
-  const uint32_t npairs = blk.w >> 2, height = blk.h, stride = blk.stride;
-  uint32_t* dst = coef + blk.dst_off;
-  uint32_t* gw = s_g + threadIdx.x;
-  const uint32_t mmsbp2 = blk.missing_msbs + 2u;
-  const uint32_t p = 30u - blk.missing_msbs;
-  const uint32_t pscale = 1u << (p - 1);
-  // integer output: ((v + 2) << (p - 1)) >> (31 - K_max) = ((v + 2) * 2^(K_max - missing_msbs - 1)) >> 1
-  const uint32_t mul_a = 1u << (blk.K_max - blk.missing_msbs - 1u);
-  const float delta = blk.delta;
-  uint32_t fail = 0;
-  for (uint32_t j = 0; j <= 16; ++j) gw[j * DEC1_THREADS] = 0;
-  uint32_t sg_lo = 0, sg_hi = 0;              // bottom-sample significance of the row above: bit 2q = left, 2q+1 = right
-
-  for (uint32_t y = 0; y < height; y += 2) {
-    const bool first = (y == 0);
-    const uint16_t* vtab = first ? T.vlc0 : T.vlc1;
-    const uint16_t* utab = first ? T.uvlc0 : T.uvlc1;
-    uint32_t* r0 = dst + (size_t)y * stride;
-    uint32_t* r1 = r0 + stride;
-    uint32_t rho_left = 0;
-    uint32_t rs_lo = sg_lo, rs_hi = sg_hi, rs_carry = 0;      // row-above significance, walked 4 bits per pair
-    uint32_t cu_lo = 0, cu_hi = 0;                            // this row's, built from the top down
-    uint32_t wj = gw[0];                                      // row-above exponent words: pair j, then pair j + 1
-    uint32_t h_carry = 0;                                     // h of the bottom-right sample of the quad to the left
-    #pragma unroll 1
-    for (uint32_t j = 0; j < npairs; ++j) {
-      while (vlc.bits <= 32) rev_fill32(vlc);                 // the pair reads at most 2 x 7 + 6 + 10 bits
-      uint32_t vt = (uint32_t)vlc.tmp, vused = 0;
-      const uint32_t wj1 = gw[(j + 1) * DEC1_THREADS];
-      // bit 0: right of quad 2j-1, 1: left of 2j, 2: right of 2j, 3: left of 2j+1, 4: right of 2j+1, 5: left of 2j+2
-      const uint32_t y6 = rs_carry | ((rs_lo & 0x1Fu) << 1);
-      const uint32_t z = y6 | (y6 >> 1);                      // bit 0: above quad 2j, bit 2: between, bit 4: beyond 2j+1
-      rs_carry = (rs_lo >> 3) & 1u;
-      rs_lo = __funnelshift_r(rs_lo, rs_hi, 4); rs_hi >>= 4;
-      uint32_t t[2];
-      #pragma unroll
-      for (uint32_t i = 0; i < 2; ++i) {
-        uint32_t c;
-        if (first) c = (rho_left & 1u) | (rho_left >> 1);
-        else c = ((z >> (2 * i)) & 5u) | (rho_left > 3u ? 2u : 0u);
-        uint32_t e = vtab[(c << 7) | (vt & 0x7Fu)];
-        if (c == 0) {               // significance of an all-zero context comes from MEL
-          run -= 2;
-          if (run != -1) e = 0;
-          if (run < 0) run = mel_next_run(mel);
-        }
-        vt >>= (e & 7u); vused += (e & 7u);
-        t[i] = e;
-        rho_left = (e >> 4) & 15u;
-      }
-      // U-VLC of the pair (:940-974 initial row, :1066-1085 others)
-      uint32_t mode = ((t[0] >> 3) & 1u) | ((t[1] >> 2) & 2u);
-      if (first && mode == 3) {
-        run -= 2;
-        if (run == -1) mode = 4;
-        if (run < 0) run = mel_next_run(mel);
-      }
-      uint32_t ent = utab[(mode << 6) | (vt & 0x3Fu)];
-      vt >>= (ent & 7u); vused += (ent & 7u);
-      ent >>= 3;
-      uint32_t len = ent & 0xFu;
-      const uint32_t suf = vt & ((1u << len) - 1u);
-      vused += len;
-      vlc.tmp >>= vused; vlc.bits -= vused;
-      ent >>= 4;
-      len = ent & 7u; ent >>= 3;
-      const uint32_t kap = first ? 1u : 0u;
-      const uint32_t uu[2] = { kap + (ent & 7u) + (suf & ~(0xFFu << len)), kap + (ent >> 3) + (suf >> len) };
-      // this row's significance bits of the pair, pushed in at the top
-      {
-        const uint32_t ta = (t[0] >> 5) & 5u, tb = (t[1] >> 5) & 5u;       // bit 0: bottom-left, bit 2: bottom-right
-        const uint32_t nb = ((ta | (ta >> 1)) & 3u) | (((tb | (tb >> 1)) & 3u) << 2);
-        cu_lo = __funnelshift_r(cu_lo, cu_hi, 4); cu_hi = (cu_hi >> 4) | (nb << 28);
-      }
-      // exponent predictor inputs of the two quads: g[2j] | g[2j+1], g[2j+1] | g[2j+2]
-      const uint32_t gor[2] = { (wj | (wj >> 16)) & 0xFFFFu, (wj >> 16) | (wj1 & 0xFFFFu) };
-      wj = wj1;
-
-      // ---- MagSgn of the two quads (:1087-1316)
-      uint32_t o[2][4], hb[2][2];
-      #pragma unroll
-      for (uint32_t i = 0; i < 2; ++i) {
-        const uint32_t inf = t[i];
-        const uint32_t rho = (inf >> 4) & 15u, ek = inf >> 12, e1 = (inf >> 8) & 15u;
-        uint32_t Uq = uu[i];
-        if (!first) Uq += (rho & (rho - 1u)) ? 32u - (uint32_t)__clz((int)(gor[i] | 1u)) : 1u;
-        fail |= (Uq > mmsbp2) ? 1u : 0u;
-        Uq = min(Uq, mmsbp2);
-        // m_n = sigma_n * (U_q - ek_n) for the four samples at once, one byte each
-        const uint32_t rb = (rho * 0x00204081u) & 0x01010101u, eb = (ek * 0x00204081u) & 0x01010101u;
-        const uint32_t mb = (Uq * 0x01010101u - eb) & (rb * 0xFFu);
-        const uint32_t m0 = mb & 0xFFu, m1 = (mb >> 8) & 0xFFu, m2 = (mb >> 16) & 0xFFu, m3 = mb >> 24;
-        while (ms.w.bits < 64) ms_fill(ms);                     // the quad reads at most 64 bits
-        const uint32_t lo = (uint32_t)ms.w.w0, hi = (uint32_t)(ms.w.w0 >> 32);
-        const uint32_t s01 = m0 + m1;                           // <= 32
-        const uint32_t lo2 = __funnelshift_rc(lo, hi, s01), hi2 = __funnelshift_rc(hi, 0u, s01);
-        const uint32_t f[4] = { lo, __funnelshift_r(lo, hi, m0), lo2, __funnelshift_r(lo2, hi2, m2) };
-        const uint32_t mm[4] = { m0, m1, m2, m3 };
-        win_drop(ms.w, s01 + m2 + m3);
-        #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint32_t m = mm[k], bits = f[k];
-          const uint32_t pw = 1u << m;
-          uint32_t v = (bits & (pw - 1u)) | 1u;
-          v = ((e1 >> k) & 1u) * pw + v;                          // bit m is clear: + is |
-          const bool sig = (rho >> k) & 1u;
-          if (k & 1) hb[i][k >> 1] = sig ? (v >> 1) : 0u;
-          uint32_t val;
-          if (MODE == 0) { const uint32_t a = (v * mul_a + 2u * mul_a) >> 1; val = a * (1u - 2u * (bits & 1u)); }   // two's complement: +a or -a
-          else {
-            const uint32_t mag = v * pscale + 2u * pscale;        // (v + 2) << (p - 1): magnitude with the half-LSB bin centre
-            if (MODE == 1) val = __float_as_uint(__fmul_rn((float)mag, delta)) | (bits << 31);
-            else val = (bits << 31) | mag;
-          }
-          o[i][k] = sig ? val : 0u;
-        }
-      }
-      gw[j * DEC1_THREADS] = (h_carry | hb[0][0]) | ((hb[0][1] | hb[1][0]) << 16);
-      h_carry = hb[1][1];
-      *reinterpret_cast<uint4*>(r0 + 4 * j) = make_uint4(o[0][0], o[0][2], o[1][0], o[1][2]);
-      *reinterpret_cast<uint4*>(r1 + 4 * j) = make_uint4(o[0][1], o[0][3], o[1][1], o[1][3]);
-    }
-    gw[npairs * DEC1_THREADS] = h_carry;                      // g[nq]: nothing to the right
-    if (fail) break;
-    // align this row's significance bits (npairs x 4 bits sit at the top of the 64-bit register)
-    {
-      const uint32_t sh = 64u - 4u * npairs;                  // 0, 4, ..., 60
-      const uint32_t a0 = sh >= 32 ? cu_hi : cu_lo, a1 = sh >= 32 ? 0u : cu_hi;
-      sg_lo = __funnelshift_r(a0, a1, sh & 31u); sg_hi = a1 >> (sh & 31u);
-    }
-  }
-  block_status[b] = fail ? DST_FAIL : 0u;
-}
-
-
-// ---- the fast path split over two threads per code-block ------------------------------------------------------
-// A code-block's cleanup pass is two chains: MEL + VLC + U-VLC decoding (each codeword's position and context depend
-// on the one before) and MagSgn extraction (positions depend on the row above through the exponent predictor).  The
-// second needs the first's results but not the other way round, so the pair runs as a producer and a consumer
-// thread in different warps of one CTA: warps 0-1 decode the quad records (rho, e_k, e_1, u) of 64 blocks one
-// quad-row ahead into a double-buffered shared-memory row, warps 2-3 read them and do what is left of the fast
-// kernel.  Hand-over per quad-row through named barriers (producers bar.arrive on FULL, consumers bar.sync; the
+// The pass is two chains: MEL + VLC + U-VLC decoding (each codeword's position and context depend on the one
+// before) and MagSgn extraction (positions depend on the row above through the exponent predictor).  The second
+// needs the first's results but not the other way round, so the pair runs as a producer and a consumer thread in
+// different warps of one CTA: warps 0-1 decode the quad records (rho, e_k, e_1, u) of 64 blocks one quad-row ahead
+// into a double-buffered shared-memory row, warps 2-3 read them, extract the MagSgn fields and store the samples.
+// Hand-over per quad-row through named barriers (producers bar.arrive on FULL, consumers bar.sync; the
 // reverse on EMPTY), no polling.  Twice the threads per block: the serial chain of a block -- which bounds the
 // kernel's duration when 49 152 blocks are all that is in flight -- is cut to the longer of the two halves.
 #define SP_BLOCKS 64
@@ -1614,28 +1094,6 @@ ht_dec_fill_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks, uint32
 
 } // namespace
 
-void launch_ht_decode(const DecBlock* blocks, uint32_t nblocks, const uint8_t* codestream,
-                      uint32_t* coef, uint32_t* scratch, const uint16_t* tables, uint32_t out_mode,
-                      uint32_t* block_status, uint32_t max_len1, cudaStream_t st)
-{
-  if (nblocks == 0) return;
-  // shared-memory budget for the de-stuffed MagSgn bits of one block (<= 8 KB per warp); larger
-  // blocks use their global scratch
-  uint32_t ms_cap_words = ((max_len1 >> 2) + 4 + 31) & ~31u;
-  if (ms_cap_words > 2048) ms_cap_words = 2048;
-  {
-    dim3 grid((nblocks + DEC1_THREADS - 1) / DEC1_THREADS), block(DEC1_THREADS);
-    OJB_LAUNCH(ht_dec_step1_kernel, grid, block, 0, st, blocks, nblocks, codestream, scratch, tables, block_status);
-  }
-  {
-    dim3 grid((nblocks + DEC_WARPS - 1) / DEC_WARPS), block(DEC_WARPS * 32);
-    size_t smem = (size_t)DEC_WARPS * ms_cap_words * 4;
-    cudaFuncSetAttribute(ht_dec_step2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(ht_dec_step2_kernel, grid, block, smem, st, blocks, nblocks, codestream, coef, scratch, out_mode, block_status,
-               ms_cap_words);
-  }
-}
-
 void launch_ht_decode_wide(const DecBlock* blocks, uint32_t nblocks, uint32_t max_width, const uint8_t* codestream,
                            uint32_t* coef, const uint16_t* tables, bool signmag, uint32_t* block_status, cudaStream_t st)
 {
@@ -1666,20 +1124,11 @@ void launch_ht_decode_serial(const DecBlock* blocks, uint32_t nblocks, uint32_t 
          : (cleanup_only && out_mode == DEC_OUT_FLOAT) ? ht_decode_serial_kernel<1> : ht_decode_serial_kernel<2>;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   dim3 grid((nblocks + DEC1_THREADS - 1) / DEC1_THREADS), block(DEC1_THREADS);
-  if (nfast) {           // blocks flagged DEC_FLAG_FAST (cleanup pass only, one output type)
-    // the producer / consumer pair by default (bench.py value 13 400-13 900 Mpixel/s with both coders split against
-    // 10 500-10 700 with one thread per block, H100 80GB HBM3 at 400 W); OJB_DEC_SPLIT=0 selects one thread per block
-    static const bool split = [] { const char* e = getenv("OJB_DEC_SPLIT"); return !(e && *e && atoi(e) == 0); }();
-    if (split) {
-      auto kf = out_mode == DEC_OUT_INT ? ht_decode_split_kernel<0> : out_mode == DEC_OUT_FLOAT ? ht_decode_split_kernel<1>
-                                                                                              : ht_decode_split_kernel<2>;
-      dim3 g2((nblocks + SP_BLOCKS - 1) / SP_BLOCKS), b2(2 * SP_BLOCKS);
-      OJB_LAUNCH(kf, g2, b2, 0, st, blocks, nblocks, codestream, coef, tables, block_status);
-    } else {
-      auto kf = out_mode == DEC_OUT_INT ? ht_decode_fast_kernel<0> : out_mode == DEC_OUT_FLOAT ? ht_decode_fast_kernel<1>
-                                                                                              : ht_decode_fast_kernel<2>;
-      OJB_LAUNCH(kf, grid, block, 0, st, blocks, nblocks, codestream, coef, tables, block_status);
-    }
+  if (nfast) {           // blocks flagged DEC_FLAG_FAST (cleanup pass only, one output type): the producer / consumer pair
+    auto kf = out_mode == DEC_OUT_INT ? ht_decode_split_kernel<0> : out_mode == DEC_OUT_FLOAT ? ht_decode_split_kernel<1>
+                                                                                            : ht_decode_split_kernel<2>;
+    dim3 g2((nblocks + SP_BLOCKS - 1) / SP_BLOCKS), b2(2 * SP_BLOCKS);
+    OJB_LAUNCH(kf, g2, b2, 0, st, blocks, nblocks, codestream, coef, tables, block_status);
   }
   if (nfast < nblocks) {
     OJB_LAUNCH(k, grid, block, smem, sg, blocks, nblocks, codestream, coef, scratch, tables, out_mode,

@@ -19,13 +19,9 @@
 #include "ojb_device.h"
 #include "ojb_kernels.h"
 #include "ojb_async.cuh"
-#include <cstdlib>
 
 namespace ojb {
 
-#ifndef OJB_CODER_MINB
-#define OJB_CODER_MINB 1
-#endif
 #define ES_THREADS 128
 #define ES_MEL_BYTES 200
 #define MEL_EXP(k) ((uint32_t)((0x5433222111000ull >> (4 * (k))) & 7ull))
@@ -236,7 +232,7 @@ ht_encode_serial_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
     blk = blocks[b]; blk.p = (uint16_t)(blk.p + k);
   } else {
     blk = blocks[bidx];
-    if (blk.flags & ENC_FLAG_FAST) return;               // coded by ht_encode_fast_kernel
+    if (blk.flags & ENC_FLAG_FAST) return;               // coded by ht_encode_split_kernel
   }
   typedef typename WordOf<WIDE>::W W;
   constexpr uint32_t WB = WIDE ? 64u : 32u, EB = WIDE ? 6u : 5u, EM = (1u << EB) - 1u;     // word bits; bits of a stored exponent
@@ -410,7 +406,7 @@ ht_encode_serial_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
   terminate_block<ES_THREADS, !COUNT>(ms, vlc, mel, mel_buf, slot, blk.slot_cap, status, results[bidx]);
 }
 
-// ---- fast path -------------------------------------------------------------------------------------------
+// ---- fast path: two threads per code-block -------------------------------------------------------------------
 // The same encoder for the blocks the host marks ENC_FLAG_FAST: width a multiple of 4 and at most 64, even
 // height, 16-byte aligned rows, K_max <= 15 (the four MagSgn fields of a quad fit 64 bits; 2 * magnitude - 1 fits
 // 16 bits), no magnitude-overflow check.  Without the per-quad bounds / width / precision tests, and with the
@@ -420,167 +416,6 @@ ht_encode_serial_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
 //     exponent of the four samples above a quad is 32 - clz(g[q] | g[q+1]) -- one CLZ instead of a 4-way max of
 //     stored exponents; inside the quad the largest exponent is 32 - clz(x0 | x1 | x2 | x3) and a sample reaches it
 //     iff x_i >> (e_max - 1) is non-zero.
-__global__ void __launch_bounds__(ES_THREADS, OJB_CODER_MINB)
-ht_encode_fast_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks,
-                      const uint32_t* __restrict__ coef, uint8_t* __restrict__ slots,
-                      EncResult* __restrict__ results, const uint16_t* __restrict__ tables,
-                      uint32_t* __restrict__ status)
-{
-  __shared__ uint16_t s_vlc[2 * 2048];
-  __shared__ uint16_t s_uvlc[36];
-  __shared__ uint32_t s_g[17 * ES_THREADS];
-
-  for (uint32_t i = threadIdx.x; i < 2 * 2048; i += blockDim.x) s_vlc[i] = tables[i];
-  if (threadIdx.x < 33) s_uvlc[threadIdx.x] = tables[2 * 2048 + threadIdx.x];
-  __syncthreads();
-
-  const uint32_t bidx = blockIdx.x * ES_THREADS + threadIdx.x;
-  if (bidx >= nblocks) return;
-  const EncBlock blk = blocks[bidx];
-  if (!(blk.flags & ENC_FLAG_FAST)) return;
-  const uint32_t npairs = blk.w >> 2, height = blk.h, stride = blk.stride, p = blk.p;
-  const uint32_t* __restrict__ src = coef + blk.src_off;
-  uint8_t* slot = slots + blk.slot_off;
-  uint2* ms_dst = reinterpret_cast<uint2*>(slot);          // slots are 16-byte aligned
-  uint32_t* vl_end = reinterpret_cast<uint32_t*>(slot + blk.slot_cap);
-  uint32_t* gw = s_g + threadIdx.x;
-  const uint32_t slot_words = blk.slot_cap >> 2;
-  // MEL bytes (a few dozen per block, at most 192) are parked inside the block's own slot, in the gap the host's
-  // sizing leaves between the MagSgn worst case and the VLC worst case, instead of 200 bytes of shared memory per
-  // thread: the kernel's footprint drops from 42 KB to 17 KB per CTA and more frames' CTAs fit on an SM
-  uint8_t* mel_buf;
-  {
-    const uint32_t nqp = ((uint32_t)(blk.w >> 1) * (uint32_t)(blk.h >> 1) + 1u) / 2u;
-    uint32_t vl_worst = (nqp * 30u + 12u + 7u) / 8u; vl_worst += vl_worst / 7u + 8u;
-    mel_buf = slot + (blk.slot_cap - vl_worst - 216u);
-  }
-  const uint32_t pm1 = p - 1u, vmask = (2u << (31u - p)) - 2u;       // p >= 16
-
-  MsWriter ms; ms.w0 = 0; ms.w1 = 0; ms.nbits = 0; ms.words = 0; ms.last_ff = 0;
-  VlcWriter vlc; vlc.acc = 0xFFFull; vlc.nbits = 12; vlc.words = 0; vlc.prev = 0;
-  MelWriter mel; mel.k = 0; mel.run = 0; mel.tmp = 0; mel.rem = 8; mel.pos = 0;
-  uint32_t any_sig = 0;
-  bool overflow = false;
-  for (uint32_t j = 0; j <= 16; ++j) gw[j * ES_THREADS] = 0;
-  uint32_t sg_lo = 0, sg_hi = 0;
-
-  for (uint32_t y = 0; y < height; y += 2) {
-    const bool first = (y == 0);
-    const uint4* r0 = reinterpret_cast<const uint4*>(src + (size_t)y * stride);
-    const uint4* r1 = reinterpret_cast<const uint4*>(src + (size_t)(y + 1) * stride);
-    const uint16_t* vtab = s_vlc + (first ? 0u : 2048u);
-    uint32_t rho_left = 0;
-    uint32_t rs_lo = sg_lo, rs_hi = sg_hi, rs_carry = 0;
-    uint32_t cu_lo = 0, cu_hi = 0;
-    uint32_t wj = gw[0], x_carry = 0;
-    uint4 na = ld_stream16(r0), nb = ld_stream16(r1);
-    #pragma unroll 1
-    for (uint32_t j = 0; j < npairs; ++j) {
-      const uint4 ca = na, cb = nb;
-      if (j + 1 < npairs) { na = ld_stream16(r0 + j + 1); nb = ld_stream16(r1 + j + 1); }   // next pair in flight while this one is coded
-      const uint32_t wj1 = gw[(j + 1) * ES_THREADS];
-      const uint32_t y6 = rs_carry | ((rs_lo & 0x1Fu) << 1);
-      const uint32_t z = y6 | (y6 >> 1);
-      rs_carry = (rs_lo >> 3) & 1u;
-      rs_lo = __funnelshift_r(rs_lo, rs_hi, 4); rs_hi >>= 4;
-      const uint32_t gor[2] = { (wj | (wj >> 16)) & 0xFFFFu, (wj >> 16) | (wj1 & 0xFFFFu) };
-      wj = wj1;
-
-      uint32_t uq[2], xb[2][2], rr[2], cwl[2];
-      unsigned long long cwd[2];
-      uint32_t pair_bits = 0, pair_len = 0;      // CxtVLC codewords of the pair, then its U-VLC bits (<= 30)
-      #pragma unroll
-      for (uint32_t h = 0; h < 2; ++h) {
-        // quad order TL, BL, TR, BR
-        const uint32_t t[4] = { h ? ca.z : ca.x, h ? cb.z : cb.x, h ? ca.w : ca.y, h ? cb.w : cb.y };
-        uint32_t rho = 0, x[4], s[4];
-        #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const uint32_t v = (t[i] >> pm1) & vmask;                // 2 * magnitude (sign and the bit below the LSB dropped)
-          const uint32_t sig = min(v, 1u);
-          rho |= sig << i;
-          x[i] = v - sig;                                          // 2 * magnitude - 1 (0 when insignificant)
-          s[i] = v - 2u + (t[i] >> 31);                            // MagSgn value 2 * (magnitude - 1) + sign
-        }
-        any_sig |= rho;
-        rr[h] = rho;
-        xb[h][0] = x[1]; xb[h][1] = x[3];
-        const uint32_t emax = 32u - (uint32_t)__clz((int)(x[0] | x[1] | x[2] | x[3]));
-        uint32_t kappa = 1, cq;
-        if (first) cq = (rho_left >> 1) | (rho_left & 1);
-        else {
-          const int me = 32 - __clz((int)gor[h]);                  // largest exponent of the four samples above
-          if (rho & (rho - 1)) kappa = (uint32_t)max(1, me - 1);
-          cq = ((z >> (2 * h)) & 5u) | (rho_left > 3u ? 2u : 0u);
-        }
-        const uint32_t Uq = max(emax, kappa);
-        const uint32_t u = Uq - kappa;
-        uq[h] = u;
-        // which samples reach the maximum exponent (only coded when u > 0)
-        // (branch-free: every x_i < 2^emax, so x_i >> (emax - 1) is 0 or 1; an empty quad has u == 0)
-        const uint32_t sh = max(emax, 1u) - 1u;
-        const uint32_t eps = ((x[0] >> sh) | ((x[1] >> sh) << 1) | ((x[2] >> sh) << 2) | ((x[3] >> sh) << 3)) & (0u - min(u, 1u));
-        const uint32_t tuple = vtab[(cq << 8) + (rho << 4) + eps];
-        pair_bits |= (tuple >> 8) << pair_len; pair_len += (tuple >> 4) & 7u;      // :661-662
-        if (cq == 0) mel_event<1>(mel, rho != 0, mel_buf);                          // :664-665
-        {                                                                         // :667-674
-          const uint32_t rb = (rho * 0x00204081u) & 0x01010101u, eb = ((tuple & 15u) * 0x00204081u) & 0x01010101u;
-          const uint32_t mb = (Uq * 0x01010101u - eb) & (rb * 0xFFu);
-          const uint32_t m0 = mb & 0xFFu, m1 = (mb >> 8) & 0xFFu, m2 = (mb >> 16) & 0xFFu, m3 = mb >> 24;
-          // fields of at most 16 bits: each column of the quad fits a word
-          const uint32_t A = (s[0] & ((1u << m0) - 1u)) | ((s[1] & ((1u << m1) - 1u)) << m0);
-          const uint32_t B = (s[2] & ((1u << m2) - 1u)) | ((s[3] & ((1u << m3) - 1u)) << m2);
-          const uint32_t la = m0 + m1, lb = m2 + m3;               // <= 32 each
-          cwd[h] = (unsigned long long)A | ((unsigned long long)B << la); cwl[h] = la + lb;
-        }
-        rho_left = rho;
-      }
-      // the two appends come after both quads have been worked out: their arithmetic is independent and
-      // overlaps, only the packing is a chain
-      ms_put(ms, cwd[0], cwl[0], ms_dst);
-      ms_put(ms, cwd[1], cwl[1], ms_dst);
-      // this row's state for the next one
-      {
-        const uint32_t ta = (rr[0] >> 1) & 5u, tb = (rr[1] >> 1) & 5u;       // bit 0: bottom-left, bit 2: bottom-right
-        const uint32_t nbits4 = ((ta | (ta >> 1)) & 3u) | (((tb | (tb >> 1)) & 3u) << 2);
-        cu_lo = __funnelshift_r(cu_lo, cu_hi, 4); cu_hi = (cu_hi >> 4) | (nbits4 << 28);
-        gw[j * ES_THREADS] = (x_carry | xb[0][0]) | ((xb[0][1] | xb[1][0]) << 16);
-        x_carry = xb[1][1];
-      }
-      // ---- U-VLC of the pair (:763-785, :985-988)
-      {
-        const uint32_t u0 = uq[0], u1 = uq[1];
-        uint32_t c0, c1;
-        if (first) {
-          if (u0 > 0 && u1 > 0) mel_event<1>(mel, min(u0, u1) > 2, mel_buf);
-          if (u0 > 2 && u1 > 2) { c0 = s_uvlc[u0 - 2]; c1 = s_uvlc[u1 - 2]; }
-          else if (u0 > 2 && u1 > 0) { c0 = s_uvlc[u0]; c1 = (u1 - 1) | (1u << 3); }     // one-bit u1
-          else { c0 = s_uvlc[u0]; c1 = s_uvlc[u1]; }
-        } else { c0 = s_uvlc[u0]; c1 = s_uvlc[u1]; }
-        uint32_t bits = pair_bits, len = pair_len;
-        bits |= (c0 & 7u) << len; len += (c0 >> 3) & 7u;
-        bits |= (c1 & 7u) << len; len += (c1 >> 3) & 7u;
-        bits |= ((c0 >> 6) & 31u) << len; len += (c0 >> 11) & 31u;
-        bits |= ((c1 >> 6) & 31u) << len; len += (c1 >> 11) & 31u;
-        vlc_put(vlc, bits, len, vl_end);
-      }
-    }
-    gw[npairs * ES_THREADS] = x_carry;
-    {
-      const uint32_t sh = 64u - 4u * npairs;
-      const uint32_t a0 = sh >= 32 ? cu_hi : cu_lo, a1 = sh >= 32 ? 0u : cu_hi;
-      sg_lo = __funnelshift_r(a0, a1, sh & 31u); sg_hi = a1 >> (sh & 31u);
-    }
-    if (ms.words + vlc.words + 24 >= slot_words) { overflow = true; break; }
-  }
-
-  if (overflow) { atomicOr(status, 1u); results[bidx].len_head = 0; results[bidx].len_tail = 0; return; }
-  if (any_sig == 0) { results[bidx].len_head = 0; results[bidx].len_tail = 0; return; }   // block not included
-  terminate_block<1>(ms, vlc, mel, mel_buf, slot, blk.slot_cap, status, results[bidx]);
-}
-
-
-// ---- the fast path split over two threads per code-block ---------------------------------------------------
 // Thread A of a block (warps 0-1 of the CTA) does everything that touches the samples: magnitudes, exponents,
 // contexts, the CxtVLC table look-up, and the MagSgn stream; per quad pair it hands thread B (warps 2-3) one word
 // -- the pair's CxtVLC bits and length, the two u_q, and which MEL events the pair produces -- through a
@@ -804,14 +639,9 @@ void launch_ht_encode_serial(const EncBlock* blocks, uint32_t nblocks, uint32_t 
   cudaFuncSetAttribute(ht_encode_serial_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   cudaFuncSetAttribute(ht_encode_serial_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   dim3 grid((nblocks + ES_THREADS - 1) / ES_THREADS), block(ES_THREADS);
-  if (nfast) {
-    // the two-thread split by default (see launch_ht_decode_serial); OJB_ENC_SPLIT=0 selects one thread per block
-    static const bool split = [] { const char* e = getenv("OJB_ENC_SPLIT"); return !(e && *e && atoi(e) == 0); }();
-    if (split) {
-      dim3 g2((nblocks + SE_BLOCKS - 1) / SE_BLOCKS), b2(2 * SE_BLOCKS);
-      OJB_LAUNCH(ht_encode_split_kernel, g2, b2, 0, st, blocks, nblocks, coef, slots, results, tables, status);
-    } else
-      OJB_LAUNCH(ht_encode_fast_kernel, grid, block, 0, st, blocks, nblocks, coef, slots, results, tables, status);
+  if (nfast) {           // blocks flagged ENC_FLAG_FAST: two threads per block
+    dim3 g2((nblocks + SE_BLOCKS - 1) / SE_BLOCKS), b2(2 * SE_BLOCKS);
+    OJB_LAUNCH(ht_encode_split_kernel, g2, b2, 0, st, blocks, nblocks, coef, slots, results, tables, status);
   }
   if (wide)
     OJB_LAUNCH(ht_encode_serial_kernel<true>, grid, block, smem, st, blocks, nblocks, coef, slots, results, tables, status,

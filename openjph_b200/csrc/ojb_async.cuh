@@ -20,8 +20,8 @@ template <int N> __device__ __forceinline__ void cp_async(void* dst, const void*
 // A 16-byte load from a per-thread stream of coefficients (the block encoders for the common shape: one thread reads a code-block's
 // samples, 49 152 blocks in an 8K frame, each of the two rows of a quad row 16 bytes at a time).  On an L2 miss the .L2::128B hint has L2 fetch the whole
 // aligned 128 bytes that the same thread reads next, so DRAM sees 128-byte requests rather than scattered 32-byte
-// sectors: ht_encode_fast_kernel 1.37-1.43 ms against 1.48-1.51 ms per 8K frame on an H100 80GB HBM3 at 400 W (the
-// 256-byte hint measured 1.42 ms; four frames in one launch were slower, DESIGN §3).
+// sectors: the one-thread-per-block encoder of the common shape took 1.37-1.43 ms against 1.48-1.51 ms per 8K frame on an
+// H100 80GB HBM3 at 400 W (the 256-byte hint measured 1.42 ms; four frames in one launch were slower, DESIGN §3).
 __device__ __forceinline__ uint4 ld_stream16(const uint4* p) {
   uint4 v;
   asm("ld.global.nc.L2::128B.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));

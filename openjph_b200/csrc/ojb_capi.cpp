@@ -700,7 +700,7 @@ int ojb_decode_blocks(const uint8_t* bytes, uint64_t n_bytes, ojb_block_desc* de
     cuda_check(cudaMemcpy(d_t.p, tb.data(), tb.size() * 2, cudaMemcpyHostToDevice), "tables");
     std::vector<DecBlock> db(n);
     size_t scratch = 0;
-    uint32_t max_len1 = 0, nfast = 0;
+    uint32_t nfast = 0;
     for (uint32_t i = 0; i < n; ++i) {
       DecBlock& d = db[i]; memset(&d, 0, sizeof(d));
       d.data_off = desc[i].byte_off; d.dst_off = desc[i].sample_off; d.stride = desc[i].stride;
@@ -708,9 +708,7 @@ int ojb_decode_blocks(const uint8_t* bytes, uint64_t n_bytes, ojb_block_desc* de
       d.missing_msbs = (uint8_t)desc[i].missing_msbs; d.num_passes = (uint8_t)desc[i].num_passes;
       d.K_max = (uint8_t)(desc[i].missing_msbs + 1); d.flags = desc[i].causal ? 1 : 0;
       uint32_t nq = (d.w + 1u) / 2, qs = (nq + 1) & ~1u, nqr = (d.h + 1u) / 2;
-      scratch = (scratch + 3) & ~(size_t)3;
-      d.scratch_off = scratch; scratch += (size_t)qs * nqr + (((d.len1 + 3) / 4 + 4 + 3) & ~3u);
-      max_len1 = std::max(max_len1, d.len1);
+      d.scratch_off = scratch; scratch += (size_t)qs * nqr;        // quad records (even: 8-byte aligned)
       if (!getenv("OJB_NO_FAST_BLOCKS") && dec_block_is_fast(d)) { d.flags |= DEC_FLAG_FAST; ++nfast; }
     }
     d_b.reserve(n * sizeof(DecBlock)); d_o.reserve((n_words + 64) * 4); d_sc.reserve((scratch + 64) * 4); d_st.reserve(n * 4 + 16);
@@ -718,12 +716,8 @@ int ojb_decode_blocks(const uint8_t* bytes, uint64_t n_bytes, ojb_block_desc* de
     cuda_check(cudaMemcpy(d_o.p, samples, n_words * 4, cudaMemcpyHostToDevice), "out init");
     uint32_t maxw = 4;
     for (uint32_t i = 0; i < n; ++i) maxw = std::max(maxw, desc[i].w);
-    if (serial_block_decoder() || maxw > 64)
-      launch_ht_decode_serial(d_b.as<DecBlock>(), n, nfast, maxw, d_cs.as<uint8_t>(), d_o.as<uint32_t>(), d_sc.as<uint32_t>(),
-                              d_t.as<uint16_t>(), DEC_OUT_SIGNMAG, false, d_st.as<uint32_t>(), 0);
-    else
-      launch_ht_decode(d_b.as<DecBlock>(), n, d_cs.as<uint8_t>(), d_o.as<uint32_t>(), d_sc.as<uint32_t>(),
-                       d_t.as<uint16_t>(), DEC_OUT_SIGNMAG, d_st.as<uint32_t>(), max_len1, 0);
+    launch_ht_decode_serial(d_b.as<DecBlock>(), n, nfast, maxw, d_cs.as<uint8_t>(), d_o.as<uint32_t>(), d_sc.as<uint32_t>(),
+                            d_t.as<uint16_t>(), DEC_OUT_SIGNMAG, false, d_st.as<uint32_t>(), 0);
     cuda_check(cudaDeviceSynchronize(), "ht_decode");
     cuda_check(cudaGetLastError(), "ht_decode");
     cuda_check(cudaMemcpy(samples, d_o.p, n_words * 4, cudaMemcpyDeviceToHost), "samples");

@@ -35,10 +35,6 @@ bool serial_block_encoder() {
   static const bool v = [] { const char* e = getenv("OJB_BLOCK_ENCODER"); return !(e && strcmp(e, "warp") == 0); }();
   return v;
 }
-bool serial_block_decoder() {
-  static const bool v = [] { const char* e = getenv("OJB_BLOCK_DECODER"); return !(e && strcmp(e, "twostep") == 0); }();
-  return v;
-}
 
 CodecBase::CodecBase() {
   CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
@@ -1157,19 +1153,19 @@ void Decoder::read_headers(const uint8_t* data, size_t len, uint32_t sample_type
               d.stride = bg.plane_stride; d.w = (uint16_t)r.w; d.h = (uint16_t)r.h;
               d.K_max = (uint8_t)bg.K_max; d.delta = bg.delta;
               d.flags = (params.stripe_causal(tc.comp) ? 1u : 0u) | (params.reversible(tc.comp) ? 0u : 2u);
-              // quad records + de-stuffed MagSgn (a cleanup segment is < 65535 bytes; sized per frame)
+              // quad records of the refinement passes (an even number of words: 8-byte aligned)
               uint32_t nq = (r.w + 1) / 2, qs = (nq + 1) & ~1u, nqr = (r.h + 1) / 2;
               d.scratch_off = scratch;
-              scratch += (size_t)qs * nqr;      // MagSgn words are appended per frame
+              scratch += (size_t)qs * nqr;
             }
         }
+  d_scratch.reserve((scratch + 64) * 4);
   coded.assign(layout.num_blocks, CodedBlock());
   block_static.assign(layout.num_blocks, DecStatic());
   for (size_t b = 0; b < h_dec_proto.size(); ++b) {
     const DecBlock& d = h_dec_proto[b];
     DecStatic& g = block_static[b];
-    const uint32_t nq = (d.w + 1u) / 2, qs = (nq + 1) & ~1u, nqr = (d.h + 1u) / 2;
-    g.quad_words = qs * nqr; g.flags = d.flags; g.K_max = d.K_max;
+    g.flags = d.flags; g.K_max = d.K_max;
     DecBlock t = d; t.num_passes = 1; t.len1 = 2; t.missing_msbs = 0; t.K_max = 1;       // the frame's part of the test set to "yes"
     g.fast_shape = dec_block_is_fast(t) ? 1 : 0;
   }
@@ -1178,7 +1174,6 @@ void Decoder::read_headers(const uint8_t* data, size_t len, uint32_t sample_type
   if (!h_dec_proto.empty())
     CK(cudaMemcpy(d_proto.p, h_dec_proto.data(), h_dec_proto.size() * sizeof(DecBlock), cudaMemcpyHostToDevice));
   h_dyn.reserve(std::max<size_t>(1, h_dec_proto.size()) * sizeof(DecDyn));
-  h_scr.reserve(std::max<size_t>(1, h_dec_proto.size()) * sizeof(uint64_t));
   any_rev_blocks = any_irv_blocks = false;
   for (const DecBlock& d : h_dec_proto) { if (d.flags & 2) any_irv_blocks = true; else any_rev_blocks = true; }
   d_bstatus.reserve(std::max<size_t>(1, h_dec_proto.size()) * 4);
@@ -1337,19 +1332,14 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool plan
   }
   uint32_t nb = (uint32_t)h_dec_proto.size();
   DecDyn* hy = h_dyn.as<DecDyn>();
-  uint64_t* hs = h_scr.as<uint64_t>();
-  size_t scratch_fixed = 0;
-  if (nb) { const DecBlock& l = h_dec_proto[nb - 1]; uint32_t nq = (l.w + 1u) / 2, qs = (nq + 1) & ~1u; scratch_fixed = l.scratch_off + (size_t)qs * ((l.h + 1u) / 2); }
-  size_t scratch = scratch_fixed;
-  uint32_t max_len1 = 0, nfast = 0;
+  uint32_t nfast = 0;
   bool cleanup_only = true;                 // lets the block decoder be specialised
   const uint32_t dec_out = (any_rev_blocks && any_irv_blocks) ? (uint32_t)DEC_OUT_PER_BLOCK : any_irv_blocks ? (uint32_t)DEC_OUT_FLOAT : (uint32_t)DEC_OUT_INT;
   const bool fast_ok = dec_out != DEC_OUT_PER_BLOCK && !no_fast_blocks && !wide;
   // the frame's part of every block record (the geometry part sits in d_proto): lengths, passes, missing msbs, where
-  // the bytes are, and whether the block goes through the specialised kernel (one output type per launch).  Scratch
-  // (quad records + de-stuffed MagSgn of the general / two-step kernels) is laid out per frame.
-  // (the geometry a block's record needs here -- quad-record words, static flags, whether its shape suits the
-  // specialised kernel -- sits in 8 bytes per block, block_static, instead of the 48-byte DecBlock prototype)
+  // the bytes are, and whether the block goes through the specialised kernel (one output type per launch).
+  // (the geometry a block's record needs here -- static flags, whether its shape suits the specialised kernel --
+  // sits in 4 bytes per block, block_static, instead of the 48-byte DecBlock prototype)
   const bool masked = !block_wanted.empty(), restricted = skip_read > 0;
   const DecStatic* bst = block_static.data();
   for (uint32_t b = 0; b < nb; ++b) {
@@ -1363,10 +1353,6 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool plan
       np = 0; len1 = len2 = 0;
       if (block_res[b] < skip_recon) skip = true;            // ... and not even needed: nothing to fill
     }
-    scratch = (scratch + 3) & ~(size_t)3;
-    hs[b] = scratch;
-    scratch += (size_t)(skip ? 0u : g.quad_words) + (((len1 + 3) / 4 + 4 + 3) & ~3u);
-    max_len1 = std::max(max_len1, len1);
     if (np > 1) cleanup_only = false;
     uint32_t flags = g.flags;
     // dec_block_is_fast(): the shape part is g.fast_shape, the frame's part is checked here
@@ -1375,27 +1361,20 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool plan
     y.num_passes = (uint8_t)np; y.missing_msbs = (uint8_t)mm; y.flags = (uint8_t)flags; y.skip = skip ? 1 : 0;
     hy[b] = y;
   }
-  d_scratch.reserve((scratch + 64) * 4);
-  // scratch offsets are only read by blocks outside the specialised kernel
-  const bool need_scratch = nfast < nb || !(serial_block_decoder() || max_block_w > 64);
   host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
   if (getenv("OJB_PARSE_PROF")) fprintf(stderr, "decode host: parse %.3f ms, records %.3f ms\n", std::chrono::duration<double, std::milli>(host_t1 - host_t0).count(), host_ms - std::chrono::duration<double, std::milli>(host_t1 - host_t0).count());
   auto enqueue = [&] {
   mark(2);
-  if (nb) { launch_dec_merge(d_dec.as<DecBlock>(), d_proto.as<DecBlock>(), hy, need_scratch ? hs : nullptr, nb, stream); ++last_launches; }
+  if (nb) { launch_dec_merge(d_dec.as<DecBlock>(), d_proto.as<DecBlock>(), hy, nb, stream); ++last_launches; }
   if (wide) {
     if (!cleanup_only) fail(0x000B0009, "SigProp / MagRef passes are not implemented on the 64-bit coefficient path");
     launch_ht_decode_wide(d_dec.as<DecBlock>(), nb, max_block_w, cs_dev, d_coef.as<uint32_t>(), d_tables_dec.as<uint16_t>(), false,
                           d_bstatus.as<uint32_t>(), stream);
-  } else if (serial_block_decoder() || max_block_w > 64)
+  } else
     launch_ht_decode_serial(d_dec.as<DecBlock>(), nb, nfast, max_block_w, cs_dev, d_coef.as<uint32_t>(), d_scratch.as<uint32_t>(),
                             d_tables_dec.as<uint16_t>(), dec_out, cleanup_only,
                             d_bstatus.as<uint32_t>(), stream, &side);
-  else
-    launch_ht_decode(d_dec.as<DecBlock>(), nb, cs_dev, d_coef.as<uint32_t>(), d_scratch.as<uint32_t>(),
-                     d_tables_dec.as<uint16_t>(), (uint32_t)DEC_OUT_PER_BLOCK,
-                     d_bstatus.as<uint32_t>(), max_len1, stream);
-  last_launches += (serial_block_decoder() || max_block_w > 64) ? 1 + (nfast ? 1 : 0) + (nfast < nb ? 1 : 0) : 2;
+  last_launches += 1 + (nfast ? 1 : 0) + (nfast < nb ? 1 : 0);
   mark(3);
   if (nb) { launch_ctrl_copy(h_bstatus.p, d_bstatus.p, (size_t)nb * 4, stream); ++last_launches; }
   // synthesis, coarsest level first
@@ -1430,8 +1409,7 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool plan
   // frame's own data (block records, lengths, offsets) reaches the kernels through the pinned record buffer
   if (planes == nullptr && dev_cs != nullptr)
     run_frame({ (uint64_t)(size_t)cs_dev, (uint64_t)nb, (uint64_t)(nfast != 0), (uint64_t)(nfast < nb), (uint64_t)cleanup_only, (uint64_t)dec_out,
-                (uint64_t)need_scratch, (uint64_t)(size_t)d_scratch.p, (uint64_t)max_len1 * (serial_block_decoder() || max_block_w > 64 ? 0 : 1),
-                (uint64_t)skip_recon, (uint64_t)(size_t)hy, (uint64_t)(size_t)d_coef.p, (uint64_t)(size_t)d_image.p }, enqueue);
+                (uint64_t)(size_t)d_scratch.p, (uint64_t)skip_recon, (uint64_t)(size_t)hy, (uint64_t)(size_t)d_coef.p, (uint64_t)(size_t)d_image.p }, enqueue);
   else enqueue();
   CK(cudaStreamSynchronize(stream));
   CK(cudaGetLastError());

@@ -178,12 +178,9 @@ struct FrameInfo {
   uint32_t nlt_type[16];
 };
 
-// block-coder variants, identical results.  Encoder: the thread-per-block family by default (blocks of the
-// common shape split over two threads, OJB_ENC_SPLIT=0 keeps them on one), OJB_BLOCK_ENCODER=warp selects one
-// warp per block.  Decoder: the same family (producer / consumer pair for the common shape, OJB_DEC_SPLIT=0 for
-// one thread), OJB_BLOCK_DECODER=twostep selects step 1 (thread per block) + step 2 (warp per block).
+// block-encoder variants, identical results: the thread-per-block family by default (blocks of the common shape
+// split over two threads), OJB_BLOCK_ENCODER=warp selects one warp per block.
 bool serial_block_encoder();
-bool serial_block_decoder();
 
 class Decoder : public CodecBase {
 public:
@@ -213,12 +210,12 @@ public:
   std::vector<uint8_t> header_sig;     // bytes of the main header the geometry was built for
   std::vector<CodedBlock> coded;
   std::vector<DecBlock> h_dec_proto;   // geometry part of DecBlock, per block
-  // what the per-frame record loop of decode() needs of it: quad-record words (scratch), static flags, K_max, and
-  // whether the block's shape qualifies for ht_decode_fast_kernel (dec_block_is_fast minus the frame's fields)
-  struct DecStatic { uint32_t quad_words = 0; uint8_t flags = 0, K_max = 0, fast_shape = 0, pad = 0; };
+  // what the per-frame record loop of decode() needs of it: static flags, K_max, and whether the block's shape
+  // qualifies for ht_decode_split_kernel (dec_block_is_fast minus the frame's fields)
+  struct DecStatic { uint8_t flags = 0, K_max = 0, fast_shape = 0, pad = 0; };
   std::vector<DecStatic> block_static;
   DeviceBuf d_cs, d_dec, d_proto, d_scratch, d_bstatus;
-  PinnedBuf h_dyn, h_scr, h_bstatus;
+  PinnedBuf h_dyn, h_bstatus;
   bool any_rev_blocks = false, any_irv_blocks = false;
   void parse_tiles();
 };

@@ -55,7 +55,7 @@ struct EncBlock {
 // significant) instead of being skipped.  It happens with zero decompositions and no colour transform
 // (K_max = B - 1 + guard for the single band) for the most negative sample value.
 #define ENC_CHECK_NEGZERO 1u
-// EncBlock::flags bit 1: the block qualifies for ht_encode_fast_kernel
+// EncBlock::flags bit 1: the block qualifies for ht_encode_split_kernel
 #define ENC_FLAG_FAST 2u
 inline bool enc_block_is_fast(const EncBlock& e) {
   return e.w >= 4 && e.w <= 64 && (e.w & 3) == 0 && e.h >= 2 && (e.h & 1) == 0 && ((e.src_off | e.stride) & 3u) == 0 &&
@@ -99,7 +99,7 @@ struct RcTables {
 struct DecBlock {
   uint64_t data_off;    // byte offset of the coded bytes in the codestream buffer
   uint64_t dst_off;     // word offset of sample (0,0) in the coefficient arena
-  uint64_t scratch_off; // word offset of this block's scratch (quad records, destuffed MagSgn)
+  uint64_t scratch_off; // word offset of this block's quad records in the scratch area (blocks with SPP / MRP)
   uint32_t len1, len2;  // cleanup bytes, SPP+MRP bytes
   uint32_t stride;      // words between rows of dst
   uint16_t w, h;
@@ -113,7 +113,7 @@ struct DecDyn {
   uint16_t len1, len2;
   uint8_t num_passes, missing_msbs, flags, skip;       // skip: the block is not needed at all (w = h = 0)
 };
-// DecBlock::flags bit 2, set by the host per frame: the block qualifies for ht_decode_fast_kernel
+// DecBlock::flags bit 2, set by the host per frame: the block qualifies for ht_decode_split_kernel
 #define DEC_FLAG_FAST 4u
 inline bool dec_block_is_fast(const DecBlock& d) {
   return d.num_passes == 1 && d.len1 >= 2 && d.w >= 4 && d.w <= 64 && (d.w & 3) == 0 && d.h >= 2 && (d.h & 1) == 0 &&

@@ -20,23 +20,17 @@ void launch_ht_encode_serial(const EncBlock* blocks, uint32_t nblocks, uint32_t 
                              uint8_t* slots, EncResult* results, const uint16_t* tables, uint32_t* status,
                              cudaStream_t st, bool wide = false, const SideStream* side = nullptr);
 
-// HT decoder (ht_decode.cu): step 1 = MEL/VLC chain, one THREAD per code-block; step 2 =
-// MagSgn (+SPP +MRP) one WARP per code-block.
+// HT decoder (ht_decode.cu): one THREAD per code-block for the whole cleanup pass (+ SPP + MRP, + a zero-fill
+// kernel); nfast of the blocks carry DEC_FLAG_FAST (see dec_block_is_fast) and go through the specialised kernel.
+// scratch: the quad records of blocks with refinement passes, at DecBlock::scratch_off.
 // tables: uint16 dec_vlc[2][1024], dec_uvlc0[320], dec_uvlc1[256]
-void launch_ht_decode(const DecBlock* blocks, uint32_t nblocks, const uint8_t* codestream,
-                      uint32_t* coef, uint32_t* scratch, const uint16_t* tables, uint32_t out_mode,
-                      uint32_t* block_status, uint32_t max_len1, cudaStream_t st);
-
-// the same decoder with one THREAD per code-block for the whole cleanup pass (+ a zero-fill kernel); nfast of the
-// blocks carry DEC_FLAG_FAST (see dec_block_is_fast) and go through the specialised kernel
 void launch_ht_decode_serial(const DecBlock* blocks, uint32_t nblocks, uint32_t nfast, uint32_t max_width, const uint8_t* codestream,
                              uint32_t* coef, uint32_t* scratch, const uint16_t* tables, uint32_t out_mode,
                              bool cleanup_only, uint32_t* block_status, cudaStream_t st, const SideStream* side = nullptr);
 
-// per-frame block records: blocks[b] = proto[b] with the frame's fields (dyn, and scratch offsets when given) applied.
-// dyn / scratch_off may be mapped pinned host memory (read by the SMs, like launch_ctrl_copy)
-void launch_dec_merge(DecBlock* blocks, const DecBlock* proto, const DecDyn* dyn, const uint64_t* scratch_off,
-                      uint32_t nblocks, cudaStream_t st);
+// per-frame block records: blocks[b] = proto[b] with the frame's fields (dyn) applied.
+// dyn may be mapped pinned host memory (read by the SMs, like launch_ctrl_copy)
+void launch_dec_merge(DecBlock* blocks, const DecBlock* proto, const DecDyn* dyn, uint32_t nblocks, cudaStream_t st);
 
 // 64-bit samples (precision beyond 32 bits): cleanup pass only, output int64 (or the raw sign-magnitude words)
 void launch_ht_decode_wide(const DecBlock* blocks, uint32_t nblocks, uint32_t max_width, const uint8_t* codestream,

@@ -104,12 +104,12 @@ def test_line_interface_exchange_and_pull(name, planar, emu_lib, ref):
 
 
 def test_alternate_block_coder_variants(emu_lib, ref):
-    """the non-default kernels (warp-per-block encoder, single-pass thread-per-block decoder) are selected
-    by environment variables read once per process: run a subset of this file in a child process"""
+    """the non-default warp-per-block encoder is selected by an environment variable read once per process:
+    run a subset of this file in a child process"""
     import os, subprocess, sys
     if os.environ.get("OJB_VARIANT_CHILD"):
         pytest.skip("already inside the child run")
-    env = dict(os.environ, OJB_BLOCK_ENCODER="warp", OJB_BLOCK_DECODER="twostep", OJB_VARIANT_CHILD="1")
+    env = dict(os.environ, OJB_BLOCK_ENCODER="warp", OJB_VARIANT_CHILD="1")
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-x", "-q", "--timeout", "600",
                         "-k", "cfg1_256 or odd_rgb_L5 or rgb16_noise or offsets or irv_tiles or block_"],
                        env=env, capture_output=True, text=True, cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -196,11 +196,11 @@ def test_errors_are_reported_not_swallowed(gpu_lib):
 
 @pytest.mark.gpu
 def test_alternate_block_coder_variants_gpu(gpu_lib, ref):
-    """warp-per-block encoder and single-pass thread-per-block decoder (non-default) on the device"""
+    """warp-per-block encoder (non-default) on the device"""
     import os, subprocess, sys
     if os.environ.get("OJB_VARIANT_CHILD"):
         pytest.skip("already inside the child run")
-    env = dict(os.environ, OJB_BLOCK_ENCODER="warp", OJB_BLOCK_DECODER="twostep", OJB_VARIANT_CHILD="1")
+    env = dict(os.environ, OJB_BLOCK_ENCODER="warp", OJB_VARIANT_CHILD="1")
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-x", "-q", "-m", "gpu", "--timeout", "600",
                         "-k", "block_encoder or block_decoder or cfg2 or cfg3 or odd_rgb_L5 or offsets"],
                        env=env, capture_output=True, text=True, cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

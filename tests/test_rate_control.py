@@ -382,8 +382,7 @@ def _variant_bytes(lib_kind, env, kw, frac):
     return subprocess.check_output([sys.executable, "-c", code], env=full_env, cwd=_ROOT, text=True).strip()
 
 
-VARIANTS = [{"OJB_HOST_HEADERS": "1"}, {"OJB_BLOCK_ENCODER": "warp"}, {"OJB_ENC_SPLIT": "0"}, {"OJB_NO_FAST_BLOCKS": "1"},
-            {"OJB_NO_GRAPHS": "1"}]
+VARIANTS = [{"OJB_HOST_HEADERS": "1"}, {"OJB_BLOCK_ENCODER": "warp"}, {"OJB_NO_FAST_BLOCKS": "1"}, {"OJB_NO_GRAPHS": "1"}]
 
 
 def test_rate_control_variants_emulator(emu_lib):

@@ -4,8 +4,7 @@
 # in one launch: 1/4, 1/2, 1, 2 and 4 8K frames (more frames are stacked as tiles of one canvas).  Nearly
 # flat up to one frame means chain-bound (ILP and occupancy pay); linear means throughput-bound (the
 # instruction count pays).  Then the existing coder switches, once each, against the default.
-# usage: tools/coder_probe.sh [LABEL]     OJB_LIB_PATH picks the library, MINB_LIBS="5:path 6:path" adds
-# OJB_CODER_MINB builds.  One result line per run, prefixed with LABEL.
+# usage: tools/coder_probe.sh [LABEL]     OJB_LIB_PATH picks the library.  One result line per run, prefixed with LABEL.
 L=${1:-default}
 nvidia-smi --query-gpu=name,power.limit,clocks.sm,clocks.max.sm --format=csv,noheader
 run() {      # run NAME ENV... : one profile_once.py call, stage times of the last of PN frames
@@ -26,11 +25,5 @@ run "blocks x1" PH=8192
 run "blocks x2" PH=16384 PTILE=8192
 run "blocks x4" PH=32768 PTILE=8192
 run "encoder=warp" OJB_BLOCK_ENCODER=warp
-run "enc_split=0" OJB_ENC_SPLIT=0
-run "dec_split=0" OJB_DEC_SPLIT=0
-run "decoder=twostep" OJB_BLOCK_DECODER=twostep
 run "carveout=25" OJB_SMEM_CARVEOUT=25
 run "carveout=75" OJB_SMEM_CARVEOUT=75
-for spec in $MINB_LIBS; do
-  run "coder_minb=${spec%%:*}" OJB_LIB_PATH="${spec#*:}"
-done

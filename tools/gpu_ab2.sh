@@ -1,6 +1,6 @@
 #!/bin/bash
 # A/B of environment switches on one 8K frame: stage times (CUDA events) per variant, then ncu counters of the default
-# usage: AB_VARIANTS="OJB_DEC_SPLIT=0;OJB_NO_FAST_BLOCKS=1" bash tools/gpu_ab2.sh
+# usage: AB_VARIANTS="OJB_BLOCK_ENCODER=warp;OJB_NO_FAST_BLOCKS=1" bash tools/gpu_ab2.sh
 mkdir -p gpurun_out
 : > gpurun_out/ab2.log
 IFS=';' read -ra VARS <<< "default;${AB_VARIANTS}"

@@ -26,7 +26,7 @@ def g(r, n):
         return 0.0
 
 
-fam = (("hdr_trees", "hdr_trees"), ("hdr_items", "hdr_items"), ("hdr_groups", "hdr_groups"), ("hdr_chain", "hdr_chain"), ("hdr_expand", "hdr_expand"), ("hdr_write", "hdr_write"), ("hdr_layout", "hdr_layout"), ("hdr_place", "hdr_place"), ("hdr_copy", "hdr_copy"), ("ht_encode_fast", "ht_encode_fast"), ("ht_decode_fast", "ht_decode_fast"), ("dec_merge", "dec_merge"), ("ht_encode_serial", "ht_encode_serial"), ("ht_encode", "ht_encode"), ("ht_decode_serial", "ht_decode_serial"), ("ht_dec_fill", "ht_dec_fill"), ("ht_dec_step1", "ht_dec_step1"), ("ht_dec_step2", "ht_dec_step2"),
+fam = (("hdr_trees", "hdr_trees"), ("hdr_items", "hdr_items"), ("hdr_groups", "hdr_groups"), ("hdr_chain", "hdr_chain"), ("hdr_expand", "hdr_expand"), ("hdr_write", "hdr_write"), ("hdr_layout", "hdr_layout"), ("hdr_place", "hdr_place"), ("hdr_copy", "hdr_copy"), ("ht_encode_split", "ht_encode_split"), ("ht_decode_split", "ht_decode_split"), ("dec_merge", "dec_merge"), ("ht_encode_serial", "ht_encode_serial"), ("ht_encode", "ht_encode"), ("ht_decode_serial", "ht_decode_serial"), ("ht_dec_fill", "ht_dec_fill"),
        ("gather_blocks", "gather_blocks"), ("assemble_kernel", "assemble"), ("ctrl_copy", "ctrl_copy"),
        ("dwt_fwd_stream", "dwt_fwd"), ("dwt_inv_stream", "dwt_inv"))
 res = {}
