@@ -705,12 +705,16 @@ ht_decode_split_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
   __shared__ uint32_t s_vring[VLC_RING * SP_BLOCKS];
   __shared__ uint2 s_mring[VLC_RING * SP_BLOCKS];
   __shared__ uint32_t s_g[17 * SP_BLOCKS];
-  __shared__ uint2 s_rec[2 * 16 * SP_BLOCKS];               // [stage][pair][block]: the quad records of one quad-row
-  __shared__ uint32_t s_rows;
+  // [stage][pair][block]: the quad records of one quad-row, 16 bits per quad: bits 4-15 of the CxtVLC entry (rho, e_1,
+  // e_k) and u_q - kappa in bits 0-3 (a larger u_q sets the block's bit in s_ufail)
+  __shared__ uint32_t s_rec[2 * 16 * SP_BLOCKS];
+  __shared__ uint4 s_stage[8 * SP_BLOCKS];                  // [row * 4 + pair][block ^ (row * 4 + pair)]: see the consumer
+  __shared__ uint32_t s_rows, s_ufail[SP_BLOCKS / 32];
   {
     uint16_t* d = reinterpret_cast<uint16_t*>(&T);
     for (uint32_t i = threadIdx.x; i < sizeof(DecTables) / 2; i += blockDim.x) d[i] = tables[i];
   }
+  if (threadIdx.x < SP_BLOCKS / 32) s_ufail[threadIdx.x] = 0;
   if (threadIdx.x == 0) s_rows = 0;
   __syncthreads();
   const bool producer = threadIdx.x < SP_BLOCKS;
@@ -753,8 +757,8 @@ ht_decode_split_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
         const bool first = (r == 0);
         const uint16_t* vtab = first ? T.vlc0 : T.vlc1;
         const uint16_t* utab = first ? T.uvlc0 : T.uvlc1;
-        uint2* out = s_rec + (size_t)(r & 1) * 16 * SP_BLOCKS + tid;
-        uint32_t rho_left = 0;
+        uint32_t* out = s_rec + (size_t)(r & 1) * 16 * SP_BLOCKS + tid;
+        uint32_t rho_left = 0, ubig = 0;
         uint32_t rs_lo = sg_lo, rs_hi = sg_hi, rs_carry = 0;
         uint32_t cu_lo = 0, cu_hi = 0;
         #pragma unroll 1
@@ -796,15 +800,17 @@ ht_decode_split_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
           vlc.tmp >>= vused; vlc.bits -= vused;
           ent >>= 4;
           len = ent & 7u; ent >>= 3;
-          const uint32_t kap = first ? 1u : 0u;
-          const uint32_t u0 = kap + (ent & 7u) + (suf & ~(0xFFu << len)), u1 = kap + (ent >> 3) + (suf >> len);
+          const uint32_t u0 = (ent & 7u) + (suf & ~(0xFFu << len)), u1 = (ent >> 3) + (suf >> len);   // u_q without kappa
           {
             const uint32_t ta = (t[0] >> 5) & 5u, tb = (t[1] >> 5) & 5u;
             const uint32_t nb = ((ta | (ta >> 1)) & 3u) | (((tb | (tb >> 1)) & 3u) << 2);
             cu_lo = __funnelshift_r(cu_lo, cu_hi, 4); cu_hi = (cu_hi >> 4) | (nb << 28);
           }
-          out[j * SP_BLOCKS] = make_uint2(t[0] | (u0 << 16), t[1] | (u1 << 16));
+          ubig |= u0 | u1;
+          out[j * SP_BLOCKS] = (t[0] & 0xFFF0u) | (u0 & 15u) | (((t[1] & 0xFFF0u) | (u1 & 15u)) << 16);
         }
+        // kappa >= 1, so u_q > 15 means U_q > 16 >= missing_msbs + 2: the block fails (the 4-bit field cannot carry it)
+        if (ubig > 15u) atomicOr(&s_ufail[tid >> 5], 1u << (tid & 31));
         const uint32_t sh = 64u - 4u * npairs;
         const uint32_t a0 = sh >= 32 ? cu_hi : cu_lo, a1 = sh >= 32 ? 0u : cu_hi;
         sg_lo = __funnelshift_r(a0, a1, sh & 31u); sg_hi = a1 >> (sh & 31u);
@@ -829,27 +835,36 @@ ht_decode_split_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
     delta = blk.delta;
     for (uint32_t j = 0; j <= 16; ++j) gw[j * SP_BLOCKS] = 0;
   }
+  // The samples of a quad pair (16 bytes in each of two rows) go to a staging tile instead of global memory: chunk
+  // (row, pair) of block t sits at s_stage[c * SP_BLOCKS + (t ^ c)], c = row * 4 + pair mod 4.  Every four pairs the
+  // warp writes its 32 blocks' tiles out cooperatively, eight lanes per block (two 64-byte row pieces = four whole
+  // sectors), so a store instruction touches 8 lines instead of 32 half-sectors in 32 lines.  The XOR keeps both the
+  // owner's stores (a quarter-warp = 8 consecutive blocks, one chunk) and the write-out's loads (one block, 8 chunks)
+  // on 8 different 16-byte bank groups.  Chunks of pairs a block does not have are never written out.
+  const uint32_t lane = tid & 31u, wbase = tid & ~31u;
   for (uint32_t r = 0; r < rows; ++r) {
     named_bar_sync(BAR_FULL + (r & 1), 2 * SP_BLOCKS);
-    if (r < myrows && !fail) {
-      const bool first = (r == 0);
-      const uint2* in = s_rec + (size_t)(r & 1) * 16 * SP_BLOCKS + tid;
-      uint32_t* r0 = dst + (size_t)(2 * r) * stride;
-      uint32_t* r1 = r0 + stride;
-      uint32_t wj = gw[0], h_carry = 0;
-      #pragma unroll 1
-      for (uint32_t j = 0; j < npairs; ++j) {
-        const uint2 rec = in[j * SP_BLOCKS];
+    const bool first = (r == 0);
+    const uint32_t lp = (r < myrows && !fail) ? npairs : 0u;          // pairs this lane decodes in quad-row r
+    const uint32_t wp = __reduce_max_sync(0xFFFFFFFFu, lp);
+    // for the write-out: address of row 2r (16-byte aligned) | pairs - 1, or 0 when the lane writes nothing
+    const unsigned long long rowa = lp ? reinterpret_cast<unsigned long long>(dst + (size_t)(2 * r) * stride) | (lp - 1u) : 0ull;
+    const uint32_t* in = s_rec + (size_t)(r & 1) * 16 * SP_BLOCKS + tid;
+    uint32_t wj = gw[0], h_carry = 0;
+    #pragma unroll 1
+    for (uint32_t j = 0; j < wp; ++j) {
+      if (j < lp) {
+        const uint32_t rec = in[j * SP_BLOCKS];
         const uint32_t wj1 = gw[(j + 1) * SP_BLOCKS];
         const uint32_t gor[2] = { (wj | (wj >> 16)) & 0xFFFFu, (wj >> 16) | (wj1 & 0xFFFFu) };
         wj = wj1;
         uint32_t o[2][4], hb[2][2];
         #pragma unroll
         for (uint32_t i = 0; i < 2; ++i) {
-          const uint32_t inf = (i ? rec.y : rec.x) & 0xFFFFu;
+          const uint32_t inf = (rec >> (16 * i)) & 0xFFFFu;
           const uint32_t rho = (inf >> 4) & 15u, ek = inf >> 12, e1 = (inf >> 8) & 15u;
-          uint32_t Uq = (i ? rec.y : rec.x) >> 16;
-          if (!first) Uq += (rho & (rho - 1u)) ? 32u - (uint32_t)__clz((int)(gor[i] | 1u)) : 1u;
+          uint32_t Uq = inf & 15u;
+          Uq += (!first && (rho & (rho - 1u))) ? 32u - (uint32_t)__clz((int)(gor[i] | 1u)) : 1u;
           fail |= (Uq > mmsbp2) ? 1u : 0u;
           Uq = min(Uq, mmsbp2);
           const uint32_t rb = (rho * 0x00204081u) & 0x01010101u, eb = (ek * 0x00204081u) & 0x01010101u;
@@ -882,14 +897,29 @@ ht_decode_split_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
         }
         gw[j * SP_BLOCKS] = (h_carry | hb[0][0]) | ((hb[0][1] | hb[1][0]) << 16);
         h_carry = hb[1][1];
-        *reinterpret_cast<uint4*>(r0 + 4 * j) = make_uint4(o[0][0], o[0][2], o[1][0], o[1][2]);
-        *reinterpret_cast<uint4*>(r1 + 4 * j) = make_uint4(o[0][1], o[0][3], o[1][1], o[1][3]);
+        const uint32_t c = j & 3u;
+        s_stage[c * SP_BLOCKS + (tid ^ c)] = make_uint4(o[0][0], o[0][2], o[1][0], o[1][2]);
+        s_stage[(c + 4u) * SP_BLOCKS + (tid ^ (c + 4u))] = make_uint4(o[0][1], o[0][3], o[1][1], o[1][3]);
       }
-      gw[npairs * SP_BLOCKS] = h_carry;
+      if ((j & 3u) == 3u || j + 1 == wp) {        // write out pairs j & ~3 .. j of the warp's blocks
+        __syncwarp();
+        const uint32_t c = lane & 7u, pr = (j & ~3u) + (c & 3u);          // this lane's chunk: row c >> 2, pair pr
+        #pragma unroll 1
+        for (uint32_t i = 0; i < 32; i += 4) {
+          const uint32_t bb = i + (lane >> 3);
+          const unsigned long long a = __shfl_sync(0xFFFFFFFFu, rowa, (int)bb);
+          const uint32_t sb = __shfl_sync(0xFFFFFFFFu, stride, (int)bb);
+          if (a && pr <= (uint32_t)(a & 15u))
+            *reinterpret_cast<uint4*>(reinterpret_cast<uint32_t*>(a & ~15ull) + (c >> 2) * sb + 4 * pr) =
+                s_stage[c * SP_BLOCKS + ((wbase + bb) ^ c)];
+        }
+        __syncwarp();
+      }
     }
+    if (lp) gw[npairs * SP_BLOCKS] = h_carry;
     if (r + 2 < rows) named_bar_arrive(BAR_EMPTY + (r & 1), 2 * SP_BLOCKS);
   }
-  if (active) block_status[b] = fail ? DST_FAIL : 0u;
+  if (active) block_status[b] = (fail || ((s_ufail[tid >> 5] >> (tid & 31)) & 1u)) ? DST_FAIL : 0u;
 }
 
 
