@@ -113,14 +113,6 @@ int ojb_device_count(void);
 int ojb_set_device(int device);
 void ojb_params_default(ojb_params* p);      /* the reference's defaults: 5 levels, 64x64, RPCL */
 
-/* Main header (SOC .. last marker segment before the first SOT) of the codestream these parameters
- * produce -- what codestream::write_headers emits (ojph_codestream_local.cpp:556-711), with a TLM
- * segment (param_tlm, ojph_params.cpp:2420-2470) listing the n_tileparts (tile index, Psot) pairs
- * when params->tlm is set.  Used by the writer rank of a tile-sharded encode: the tile-parts come
- * from the other GPUs, the main header is written once.  Needs no GPU. */
-int ojb_write_main_header(const ojb_params* params, const uint32_t* tilepart_tile, const uint32_t* tilepart_psot,
-                          uint32_t n_tileparts, uint8_t* out, uint64_t out_cap, uint64_t* out_len);
-
 /* pinned host memory for frame / codestream buffers (optional; any host pointer works) */
 void* ojb_host_alloc(uint64_t bytes);
 void ojb_host_free(void* p);

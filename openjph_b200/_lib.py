@@ -85,7 +85,6 @@ SYMBOLS = {
     "ojb_device_count": (_I, []),
     "ojb_set_device": (_I, [_I]),
     "ojb_params_default": (None, [C.POINTER(Params)]),
-    "ojb_write_main_header": (_I, [C.POINTER(Params), C.POINTER(_U32), C.POINTER(_U32), _U32, _VP, _U64, C.POINTER(_U64)]),
     "ojb_host_alloc": (_VP, [_U64]),
     "ojb_host_free": (None, [_VP]),
     "ojb_enc_create": (_VP, []),

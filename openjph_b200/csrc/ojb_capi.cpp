@@ -151,24 +151,6 @@ void ojb_params_default(ojb_params* p) {
 
 void ojb_params_to_internal(const ojb_params* s, Params& P) { to_params(s, P); }      // ojb_shard.cpp
 
-int ojb_write_main_header(const ojb_params* p, const uint32_t* tp_tile, const uint32_t* tp_psot, uint32_t n_tp,
-                          uint8_t* out, uint64_t out_cap, uint64_t* out_len) {
-  return guarded([&] {
-    Params P; to_params(p, P);
-    P.finalize_for_encode();
-    std::vector<uint8_t> h;
-    P.write_main_header(h, nullptr, nullptr, 0);
-    if (P.need_tlm) {
-      if (4 + 6 * (size_t)n_tp > 65535) fail(0x000500B1, "too many tile-parts for one TLM marker segment");
-      put_u16(h, M_TLM); put_u16(h, 4 + 6 * n_tp); put_u8(h, 0); put_u8(h, 0x60);
-      for (uint32_t i = 0; i < n_tp; ++i) { put_u16(h, tp_tile[i]); put_u32(h, tp_psot[i]); }
-    }
-    if (h.size() > out_cap) fail(0x000B0030, "output buffer too small: need %zu bytes, have %zu", h.size(), (size_t)out_cap);
-    memcpy(out, h.data(), h.size());
-    *out_len = h.size();
-  });
-}
-
 void* ojb_host_alloc(uint64_t bytes) { void* p = nullptr; if (cudaMallocHost(&p, (size_t)bytes) != cudaSuccess) return nullptr; return p; }
 void ojb_host_free(void* p) { if (p) cudaFreeHost(p); }
 

@@ -1,19 +1,19 @@
-"""Tile sharding of one image across the GPUs of a box (one process per GPU, torch.distributed).
+"""One image across the GPUs of a box (one process per GPU, torch.distributed): the ctypes wrapper of ojb_shard.cpp.
 
-Tiles are independent through colour transform, DWT, quantisation, block coding and packet
-formation -- the reference gives every tile its own component / resolution tree
-(src/core/codestream/ojph_codestream_local.cpp:132-168) and concatenates the tile-parts in
-tile-index order at flush (:1148-1164, tile::flush src/core/codestream/ojph_tile.cpp:584-772).
-So rank r encodes the tiles t with t % world == r as one-tile images that keep the tile's
-ABSOLUTE canvas coordinates (image offset = tile origin, tile-grid offset = the tile's grid anchor):
-precinct and code-block partitions are anchored at the canvas origin, hence the tile-part bytes
-are identical to what a single encoder produces for that tile; only Isot (the tile index in the
-SOT segment) differs and is patched.  The only collective on the path is the final gather of the
-tile-part bytes to the writer rank, which emits the main header (+TLM) once.  Decoding mirrors it:
-every rank re-wraps its tiles' tile-parts with a one-tile main header (SIZ patched, TLM dropped)
-and decodes them; the planes stay sharded or are gathered on request.
+Every rank keeps ONE encoder / decoder with the geometry of the whole image, so canvas coordinates, Isot and packet
+contents are those of a single encoder and the codestream on the writer rank is byte-identical to the one-GPU stream.
+Two partitions (NativeShard.set_partition):
+  "tiles"    rank r codes the tiles t with t % world == r (a tile mask).  Tiles are independent through colour
+             transform, DWT, quantisation, block coding and packet formation -- the reference gives every tile its own
+             component / resolution tree (src/core/codestream/ojph_codestream_local.cpp:132-168) and concatenates the
+             tile-parts in tile-index order at flush (:1148-1164).  Encode gathers the tile-parts to the writer, which
+             adds the main header (+TLM) and EOC; decode sends each rank's tile samples to the writer.
+  "regions"  every tile-component is cut into `world` row slabs, each rank reading its slab plus a halo, so a
+             single-tile image is split too; the code-block bytes go to the writer, which writes packet headers and
+             markers as one encoder does (DESIGN.md §5).
 
-Works with the NCCL backend (GPU tensors) and with gloo (CPU tensors; used by the CPU tests).
+Transport: NCCL inside the library, or callbacks over a torch.distributed process group (gloo) -- the CPU test tier's
+emulator build, and two processes on one GPU in the GPU test tier.
 """
 import ctypes as C
 import struct
@@ -21,104 +21,11 @@ import numpy as np
 from . import _lib
 from . import codestream as cs_mod
 
-SOC, SIZ, SOT, SOD, EOC, TLM = 0xFF4F, 0xFF51, 0xFF90, 0xFF93, 0xFFD9, 0xFF55
-
-
-def _ceil_div(a, b):
-    return (a + b - 1) // b
-
-
-def tile_grid(p):
-    """tile rectangles on the canvas, raster order (ojph_codestream_local.cpp:113-131)"""
-    tw = p.tile_w if p.tile_w else p.width - p.tile_off_x
-    th = p.tile_h if p.tile_h else p.height - p.tile_off_y
-    ntx = _ceil_div(p.width - p.tile_off_x, tw)
-    nty = _ceil_div(p.height - p.tile_off_y, th)
-    tiles = []
-    for ty in range(nty):
-        for tx in range(ntx):
-            gx, gy = p.tile_off_x + tx * tw, p.tile_off_y + ty * th
-            tiles.append(dict(index=ty * ntx + tx, gx=gx, gy=gy, tw=tw, th=th,
-                              x0=max(gx, p.off_x), y0=max(gy, p.off_y),
-                              x1=min(gx + tw, p.width), y1=min(gy + th, p.height)))
-    return tiles
-
-
-def tile_params(p, tile):
-    """parameters of the one-tile image that occupies `tile`'s place on the canvas"""
-    q = type(p).from_buffer_copy(p)
-    q.width, q.height = tile["x1"], tile["y1"]
-    q.off_x, q.off_y = tile["x0"], tile["y0"]
-    q.tile_w, q.tile_h = tile["tw"], tile["th"]
-    q.tile_off_x, q.tile_off_y = tile["gx"], tile["gy"]
-    q.tlm = 0
-    return q
-
-
-def crop_planes(p, planes, tile):
-    """the tile's samples of every component (components may be sub-sampled)"""
-    out = []
-    for c, a in enumerate(planes):
-        dx, dy = p.dx[c], p.dy[c]
-        ox, oy = _ceil_div(p.off_x, dx), _ceil_div(p.off_y, dy)
-        x0, x1 = _ceil_div(tile["x0"], dx) - ox, _ceil_div(tile["x1"], dx) - ox
-        y0, y1 = _ceil_div(tile["y0"], dy) - oy, _ceil_div(tile["y1"], dy) - oy
-        out.append(np.ascontiguousarray(a[y0:y1, x0:x1]))
-    return out
-
-
-def split_codestream(cs):
-    """-> (main header bytes up to the first SOT, [(Isot, tile-part bytes incl. SOT) ...])"""
-    b = memoryview(cs)
-    if len(b) < 4 or struct.unpack(">H", b[0:2])[0] != SOC:
-        raise cs_mod.OjphError("not a codestream: SOC missing")
-    pos = 2
-    while True:
-        if pos + 4 > len(b):
-            raise cs_mod.OjphError("truncated main header")
-        m, ln = struct.unpack(">HH", b[pos:pos + 4])
-        if m == SOT:
-            break
-        pos += 2 + ln
-    header = bytes(b[:pos])
-    parts = []
-    while pos + 2 <= len(b):
-        m = struct.unpack(">H", b[pos:pos + 2])[0]
-        if m == EOC:
-            break
-        if m != SOT or pos + 12 > len(b):
-            raise cs_mod.OjphError("tile-part does not start with SOT")
-        isot, psot = struct.unpack(">HI", b[pos + 4:pos + 10])
-        end = pos + psot if psot else len(b) - 2
-        if end > len(b):
-            raise cs_mod.OjphError("truncated tile-part")
-        parts.append((isot, bytes(b[pos:end])))
-        pos = end
-    return header, parts
-
-
-def _with_isot(part, t):
-    return part[:4] + struct.pack(">H", t) + part[6:]
-
-
-def one_tile_header(header, tile):
-    """main header of the one-tile image: SIZ geometry patched, TLM segments dropped"""
-    out = bytearray(header[:2])
-    pos = 2
-    while pos < len(header):
-        m, ln = struct.unpack(">HH", header[pos:pos + 4])
-        seg = bytearray(header[pos:pos + 2 + ln])
-        if m == SIZ:
-            struct.pack_into(">IIIIIIII", seg, 6, tile["x1"], tile["y1"], tile["x0"], tile["y0"],
-                             tile["tw"], tile["th"], tile["gx"], tile["gy"])
-        if m != TLM:
-            out += seg
-        pos += 2 + ln
-    return bytes(out)
+SIZ = 0xFF51
 
 
 def siz_params(header):
-    """image / tile geometry and sub-sampling out of the SIZ segment (enough for tile_grid)"""
+    """image / tile geometry and sub-sampling out of the SIZ segment (enough for comp_dims)"""
     if struct.unpack(">H", header[2:4])[0] != SIZ:
         raise cs_mod.OjphError("SIZ must follow SOC")
     x1, y1, x0, y0, tw, th, gx, gy, nc = struct.unpack(">IIIIIIIIH", header[8:42])
@@ -134,206 +41,11 @@ def siz_params(header):
     return p
 
 
-def write_main_header(p, tileparts, lib=None):
-    """main header of the whole image; tileparts = [(tile index, Psot) ...] in codestream order"""
-    L = lib if lib is not None else _lib.lib()
-    n = len(tileparts)
-    ti = (C.c_uint32 * max(1, n))(*[t for t, _ in tileparts])
-    ps = (C.c_uint32 * max(1, n))(*[l for _, l in tileparts])
-    out = np.empty(1 << 16, np.uint8)
-    ln = C.c_uint64()
-    if L.ojb_write_main_header(C.byref(p), ti, ps, n, out.ctypes.data, out.size, C.byref(ln)) != 0:
-        raise cs_mod.OjphError(L.ojb_last_error().decode(errors="replace"))
-    return out[:ln.value].tobytes()
-
-
-def my_tiles(ntiles, rank, world):
-    return [t for t in range(ntiles) if t % world == rank]
-
-
-class TileEncoders:
-    """the encoders of one rank's tiles, configured once and reused frame after frame (device arenas,
-    descriptor tables and pinned buffers are per geometry, as with codestream::restart)"""
-
-    def __init__(self, p, tiles, sample_type=cs_mod.I32, lib=None):
-        self.p, self.tiles, self.sample_type = p, list(tiles), sample_type
-        self.encs = [cs_mod.Encoder(tile_params(p, t), sample_type, lib=lib) for t in self.tiles]
-
-    def encode(self, planes):
-        """-> {tile index: [tile-part bytes ...]} for this rank's tiles of the frame"""
-        out = {}
-        for tile, enc in zip(self.tiles, self.encs):
-            _, parts = split_codestream(enc.encode(crop_planes(self.p, planes, tile)))
-            out[tile["index"]] = [_with_isot(b, tile["index"]) for _, b in parts]
-        return out
-
-    def close(self):
-        for e in self.encs:
-            e.close()
-        self.encs = []
-
-
-def encode_tiles(p, planes, tiles, sample_type=cs_mod.I32, lib=None):
-    """encode the given tiles of the image -> {tile index: [tile-part bytes ...]}"""
-    te = TileEncoders(p, tiles, sample_type, lib)
-    try:
-        return te.encode(planes)
-    finally:
-        te.close()
-
-
-def assemble(p, parts_by_tile, lib=None):
-    """main header (+TLM) + every tile's tile-parts in tile-index order + EOC"""
-    order = [(t, b) for t in sorted(parts_by_tile) for b in parts_by_tile[t]]
-    hdr = write_main_header(p, [(t, len(b)) for t, b in order], lib=lib)
-    return hdr + b"".join(b for _, b in order) + struct.pack(">H", EOC)
-
-
-# ---- collectives ---------------------------------------------------------------------------------
 def _dist():
     import torch.distributed as dist
     return dist
 
 
-def _gather_bytes(payload, dst=0, group=None):
-    """variable-length gather of byte strings to rank dst: one all_gather of the lengths, one
-    gather of the padded payloads (NCCL: device tensors, gloo: host tensors)"""
-    import torch
-    dist = _dist()
-    rank, world = dist.get_rank(group), dist.get_world_size(group)
-    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
-    n = torch.tensor([len(payload)], dtype=torch.int64, device=dev)
-    lens = [torch.zeros_like(n) for _ in range(world)]
-    dist.all_gather(lens, n, group=group)
-    lens = [int(x.item()) for x in lens]
-    cap = max(1, max(lens))
-    buf = torch.zeros(cap, dtype=torch.uint8, device=dev)
-    if payload:
-        buf[:len(payload)] = torch.from_numpy(np.frombuffer(payload, np.uint8).copy()).to(dev, non_blocking=True)
-    if rank == dst:
-        got = [torch.empty(cap, dtype=torch.uint8, device=dev) for _ in range(world)]
-        dist.gather(buf, got, dst=dst, group=group)
-        return [g[:l].cpu().numpy().tobytes() for g, l in zip(got, lens)]
-    dist.gather(buf, None, dst=dst, group=group)
-    return None
-
-
-def _pack(parts_by_tile):
-    idx = [(t, len(b)) for t in sorted(parts_by_tile) for b in parts_by_tile[t]]
-    head = struct.pack(">I", len(idx)) + b"".join(struct.pack(">II", t, l) for t, l in idx)
-    return head + b"".join(b for t in sorted(parts_by_tile) for b in parts_by_tile[t])
-
-
-def _unpack(blob):
-    n = struct.unpack(">I", blob[:4])[0]
-    idx = [struct.unpack(">II", blob[4 + 8 * i:12 + 8 * i]) for i in range(n)]
-    pos = 4 + 8 * n
-    out = {}
-    for t, l in idx:
-        out.setdefault(t, []).append(blob[pos:pos + l])
-        pos += l
-    return out
-
-
-class ShardedEncoder:
-    """one per rank: keeps the rank's tile encoders across frames; encode() is the per-frame call"""
-
-    def __init__(self, p, sample_type=cs_mod.I32, dst=0, group=None, lib=None):
-        dist = _dist()
-        self.p, self.dst, self.group, self.lib = p, dst, group, lib
-        rank, world = dist.get_rank(group), dist.get_world_size(group)
-        grid = tile_grid(p)
-        self.tiles = TileEncoders(p, [grid[t] for t in my_tiles(len(grid), rank, world)], sample_type, lib)
-
-    def encode(self, planes):
-        got = _gather_bytes(_pack(self.tiles.encode(planes)), self.dst, self.group)
-        if got is None:
-            return None
-        allp = {}
-        for blob in got:
-            allp.update(_unpack(blob))
-        return assemble(self.p, allp, lib=self.lib)
-
-    def close(self):
-        self.tiles.close()
-
-
-def encode_sharded(p, planes, sample_type=cs_mod.I32, dst=0, group=None, lib=None):
-    """every rank passes the same parameters and (at least its tiles of) the image; returns the
-    codestream on rank dst, None elsewhere.  One gather, no other communication."""
-    dist = _dist()
-    rank, world = dist.get_rank(group), dist.get_world_size(group)
-    grid = tile_grid(p)
-    mine = encode_tiles(p, planes, [grid[t] for t in my_tiles(len(grid), rank, world)], sample_type, lib)
-    got = _gather_bytes(_pack(mine), dst, group)
-    if got is None:
-        return None
-    allp = {}
-    for blob in got:
-        allp.update(_unpack(blob))
-    return assemble(p, allp, lib=lib)
-
-
-def decode_tiles(cs, tile_indices, sample_type=cs_mod.I32, lib=None, resilient=False):
-    """decode the given tiles of a codestream -> (grid, {tile index: [plane ...]})"""
-    header, parts = split_codestream(cs)
-    geo = siz_params(header)
-    grid = tile_grid(geo)
-    out = {}
-    for t in tile_indices:
-        sub = one_tile_header(header, grid[t]) + b"".join(_with_isot(b, 0) for i, b in parts if i == t) + struct.pack(">H", EOC)
-        dec = cs_mod.Decoder(resilient=resilient, lib=lib)
-        try:
-            out[t] = dec.decode(sub, sample_type)
-        finally:
-            dec.close()
-    return geo, grid, out
-
-
-def paste_tiles(geo, grid, tiles, sample_type=cs_mod.I32):
-    """full component planes from per-tile planes"""
-    dims = cs_mod.comp_dims(geo)
-    planes = [np.zeros((h, w), cs_mod._NP[sample_type]) for w, h in dims]
-    for t, tp in tiles.items():
-        tile = grid[t]
-        for c, a in enumerate(tp):
-            dx, dy = geo.dx[c], geo.dy[c]
-            ox, oy = _ceil_div(geo.off_x, dx), _ceil_div(geo.off_y, dy)
-            x0, y0 = _ceil_div(tile["x0"], dx) - ox, _ceil_div(tile["y0"], dy) - oy
-            planes[c][y0:y0 + a.shape[0], x0:x0 + a.shape[1]] = a
-    return planes
-
-
-def decode_sharded(cs, sample_type=cs_mod.I32, dst=0, group=None, lib=None, gather=True):
-    """every rank holds the codestream and decodes its tiles; with gather the full planes are
-    returned on rank dst (None elsewhere), otherwise every rank returns (geo, grid, its tiles)"""
-    dist = _dist()
-    rank, world = dist.get_rank(group), dist.get_world_size(group)
-    header, parts = split_codestream(cs)
-    ntiles = len(tile_grid(siz_params(header)))
-    geo, grid, mine = decode_tiles(cs, my_tiles(ntiles, rank, world), sample_type, lib)
-    if not gather:
-        return geo, grid, mine
-    blob = b"".join(struct.pack(">II", t, len(tp)) + b"".join(struct.pack(">II", *a.shape) + a.tobytes() for a in tp)
-                    for t, tp in sorted(mine.items()))
-    got = _gather_bytes(blob, dst, group)
-    if got is None:
-        return None
-    tiles = {}
-    dt = np.dtype(cs_mod._NP[sample_type])
-    for b in got:
-        pos = 0
-        while pos < len(b):
-            t, nc = struct.unpack(">II", b[pos:pos + 8]); pos += 8
-            tp = []
-            for _ in range(nc):
-                h, w = struct.unpack(">II", b[pos:pos + 8]); pos += 8
-                tp.append(np.frombuffer(b, dt, h * w, pos).reshape(h, w)); pos += h * w * dt.itemsize
-            tiles[t] = tp
-    return paste_tiles(geo, grid, tiles, sample_type)
-
-
-# ---- the native path: tile sharding below the C-ABI (ojb_shard.cpp) -----------------------------------------
 class NativeShard:
     """One per rank.  Wraps ojb_shard: every rank keeps one encoder / decoder with the geometry of the whole image
     and a tile mask; tile-parts (encode) and decoded tile samples (decode) go device to device to the writer rank.

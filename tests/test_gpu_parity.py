@@ -56,23 +56,6 @@ def test_line_interface_matches_frame_interface(gpu_lib, ref):
     assert order[:6] == [0, 1, 2, 0, 1, 2]                    # colour transform => interleaved default
 
 
-def test_tile_sharding_single_process(gpu_lib, ref):
-    """tiles encoded separately (as the ranks of a box do) and re-assembled == the reference codestream"""
-    from openjph_b200 import sharding
-    p = cases.make(dict(width=700, height=500, num_comps=3, bit_depth=12, num_decomps=4, reversible=True,
-                        color_transform=True, tile=(256, 256), tlm=True))
-    frame = cases.frame_for(p)
-    want = ref.encode(p, frame)
-    grid = sharding.tile_grid(p)
-    parts = {}
-    for r in range(4):
-        parts.update(sharding.encode_tiles(p, frame, [grid[t] for t in sharding.my_tiles(len(grid), r, 4)]))
-    assert sharding.assemble(p, parts) == want
-    geo, grid2, tiles = sharding.decode_tiles(want, range(len(grid)))
-    for a, b in zip(sharding.paste_tiles(geo, grid2, tiles), frame):
-        assert np.array_equal(a, b)
-
-
 def _random_blocks(rng, n, kmax_lo=1):
     bufs, descs, blks, off = [], [], [], 0
     for it in range(n):

@@ -32,6 +32,12 @@ REGION_CASES = [
 ]
 
 
+def _num_tiles(p):
+    tw = p.tile_w or p.width - p.tile_off_x
+    th = p.tile_h or p.height - p.tile_off_y
+    return -(-(p.width - p.tile_off_x) // tw) * -(-(p.height - p.tile_off_y) // th)
+
+
 def _worker(rank, world, port, q, which, gpu=False):
     sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), OJB_EMU_THREADS="2")
@@ -73,7 +79,7 @@ def _worker(rank, world, port, q, which, gpu=False):
                 # a rank reads only the rows of its slab + halo: everything else is poisoned on the other ranks
                 mine = [a.copy() for a in fr]
                 rows = sh.region_rows(0)
-                if rows is not None and len(sharding.tile_grid(p)) == 1 and p.dy[0] == 1:
+                if rows is not None and _num_tiles(p) == 1 and p.dy[0] == 1:
                     oy = -(-p.off_y // 1)
                     for a in mine[:1]:
                         a[:max(0, rows[0] - oy)] = -12345
@@ -142,8 +148,8 @@ def _run(world, which, timeout=600, gpu=False, worker=None):
     s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    procs = [ctx.Process(target=worker, args=(r, world, port, q, which)) if worker is not None else
-             ctx.Process(target=_worker, args=(r, world, port, q, which, gpu)) for r in range(world)]
+    procs = [ctx.Process(target=worker or _worker, args=(r, world, port, q, which), kwargs=dict(gpu=True) if gpu else {})
+             for r in range(world)]
     for pr in procs:
         pr.start()
     import queue
