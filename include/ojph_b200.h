@@ -153,6 +153,36 @@ void* ojb_enc_device_plane(ojb_encoder* e, uint32_t comp);
 int ojb_enc_upload_frame(ojb_encoder* e, const void* const* planes, const uint32_t* strides);
 int ojb_enc_encode_resident(ojb_encoder* e, uint8_t* out, uint64_t out_cap, uint64_t* out_len,
                             int out_on_device);
+/* ---- the image in the caller's device memory ---------------------------------------------
+ * One descriptor per frame: sample (x, y) of component c sits at
+ *   (uint8_t*)base[c] + y * row_pitch[c] + x * col_stride[c] * (sample size)
+ * in the container given to configure / read_headers (OJB_U8 / OJB_U16 / OJB_I32: 1 / 2 / 4 bytes), for the
+ * component sizes ojb_frame_info reports (comp_w / comp_h; on decode the reduced sizes after
+ * ojb_dec_restrict_input_resolution).  col_stride 1 = planar rows, 3 = RGB interleaved (HWC), 4 = RGBA, ...; so one
+ * descriptor covers CHW at any pitch, HWC, a window inside a larger canvas, a slice of a batch, and a 4-channel
+ * buffer of which only three components are coded.  The DWT kernels address the memory directly: no staging copy.
+ * Components must not overlap (not checked: the caller's responsibility); the decoder writes exactly the samples
+ * described and no other byte.
+ * Ordering: before the library reads `in` (or writes `out`) it waits on an event recorded on cuda_stream (a
+ * cudaStream_t; NULL = the legacy default stream), so work queued there before the call is complete.  The calls
+ * return with their output complete, like the frame calls.
+ * encode: the codestream goes to out (device memory when out_on_device, else host), *out_len its length.  The
+ * decode call works after ojb_dec_read_headers or ojb_dec_read_headers_device.  With the codestream in device
+ * memory on both sides, the device work of a call replays as one CUDA graph from the third call on, whatever
+ * image buffers the calls name.
+ * Errors: 0x000B003B a null base address, or a base / row pitch that is not a multiple of the sample size;
+ * 0x000B003C col_stride 0; 0x000B003D (more than one row) a row pitch smaller than one row's footprint,
+ * ((comp_w - 1) * col_stride + 1) * sample size; 0x000B003E a component spanning 4 GiB or more
+ * ((comp_h - 1) * row_pitch + footprint: offsets from base are formed in 32 bits); 0x000B003F the call came before
+ * configure / read_headers. */
+typedef struct ojb_device_image {
+  void*    base[16];       /* device address of sample (0,0) of component c */
+  uint64_t row_pitch[16];  /* bytes from one row of component c to the next */
+  uint32_t col_stride[16]; /* samples from one column to the next: 1 = planar rows, 3 = RGB HWC, 4 = RGBA ... */
+} ojb_device_image;
+int ojb_enc_encode_device(ojb_encoder* e, const ojb_device_image* in, void* cuda_stream,
+                          uint8_t* out, uint64_t out_cap, uint64_t* out_len, int out_on_device);
+int ojb_dec_decode_device(ojb_decoder* d, const ojb_device_image* out, void* cuda_stream);
 uint32_t ojb_enc_kernel_launches(ojb_encoder* e);
 /* stage times of the last encode, CUDA events on the codec's stream, milliseconds:
  * [0] H2D image  [1] DWT levels  [2] HT block encoder  [3] D2H block lengths  [4] wait + host packet

@@ -56,6 +56,11 @@ class CodingStyle(C.Structure):
     ]
 
 
+class DeviceImage(C.Structure):
+    """ojb_device_image: sample (x, y) of component c at base[c] + y * row_pitch[c] + x * col_stride[c] * sample size"""
+    _fields_ = [("base", C.c_void_p * 16), ("row_pitch", C.c_uint64 * 16), ("col_stride", C.c_uint32 * 16)]
+
+
 class Comment(C.Structure):
     _fields_ = [("data", C.c_void_p), ("len", C.c_uint16), ("rcom", C.c_uint16)]
 
@@ -102,6 +107,7 @@ SYMBOLS = {
     "ojb_enc_device_plane": (_VP, [_VP, _U32]),
     "ojb_enc_upload_frame": (_I, [_VP, C.POINTER(_VP), C.POINTER(_U32)]),
     "ojb_enc_encode_resident": (_I, [_VP, _VP, _U64, C.POINTER(_U64), _I]),
+    "ojb_enc_encode_device": (_I, [_VP, C.POINTER(DeviceImage), _VP, _VP, _U64, C.POINTER(_U64), _I]),
     "ojb_enc_kernel_launches": (_U32, [_VP]),
     "ojb_enc_num_blocks": (_U32, [_VP]),
     "ojb_enc_set_target_size": (_I, [_VP, _U64]),
@@ -122,6 +128,7 @@ SYMBOLS = {
     "ojb_dec_set_planar": (_I, [_VP, _I]),
     "ojb_dec_begin_pull": (_I, [_VP]),
     "ojb_dec_pull": (_VP, [_VP, C.POINTER(_U32)]),
+    "ojb_dec_decode_device": (_I, [_VP, C.POINTER(DeviceImage), _VP]),
     "ojb_dec_device_plane": (_VP, [_VP, _U32]),
     "ojb_dec_use_device_codestream": (_I, [_VP, _VP]),
     "ojb_dec_read_headers_device": (_I, [_VP, _VP, _U64, _U32, C.POINTER(FrameInfo)]),

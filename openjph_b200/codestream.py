@@ -100,6 +100,47 @@ def make_params(width, height, num_comps=1, bit_depth=8, is_signed=False, num_de
     return p
 
 
+def device_image(comps):
+    """an ojb_device_image from [(address, row_pitch_bytes, col_stride), ...], one entry per component"""
+    img = _lib.DeviceImage()
+    for c, (addr, pitch, col) in enumerate(comps):
+        img.base[c], img.row_pitch[c], img.col_stride[c] = addr, pitch, col
+    return img
+
+
+_TORCH_DTYPE = {U8: "uint8", U16: "uint16", I32: "int32"}
+
+
+def _tensor_image(t, layout, sample_type, dims):
+    """the ojb_device_image of a CUDA tensor: (C, H, W) for "chw", (H, W, C) for "hwc", any strides (a channels_last
+    view, batch[i], a window of a larger canvas); or a list of 2-D tensors, one per component (sub-sampled
+    components).  Components past the coded ones (an alpha channel) are left alone."""
+    import torch
+    want = getattr(torch, _TORCH_DTYPE[sample_type])
+    if isinstance(t, (list, tuple)):
+        planes = list(t)
+    else:
+        if layout not in ("chw", "hwc"):
+            raise ValueError("layout is 'chw' or 'hwc', not %r" % (layout,))
+        if t.dim() != 3:
+            raise ValueError("a %s image tensor has 3 dimensions, this one has %d" % (layout, t.dim()))
+        v = t.permute(2, 0, 1) if layout == "hwc" else t
+        planes = [v[c] for c in range(v.shape[0])]
+    if len(planes) < len(dims):
+        raise ValueError("%d components coded, the tensor holds %d" % (len(dims), len(planes)))
+    comps = []
+    for c, (w, h) in enumerate(dims):
+        p = planes[c]
+        if not p.is_cuda:
+            raise ValueError("component %d is not a CUDA tensor" % c)
+        if p.dtype != want:
+            raise ValueError("component %d is %s; the codec's sample container is %s" % (c, p.dtype, want))
+        if tuple(p.shape) != (h, w):
+            raise ValueError("component %d is %s, the codestream's is (%d, %d)" % (c, tuple(p.shape), h, w))
+        comps.append((p.data_ptr(), p.stride(0) * p.element_size(), p.stride(1)))
+    return device_image(comps)
+
+
 def comp_dims(p):
     def dc(a, b):
         return (a + b - 1) // b
@@ -220,6 +261,48 @@ class Encoder(_Base):
         self._check(self.L.ojb_enc_encode_resident(self.h, dev_ptr, cap, C.byref(n), 1))
         return int(n.value)
 
+    def encode_device(self, image, stream=0, out_ptr=None, out_cap=0):
+        """encode from device memory described by `image` (see device_image) after the work queued on the CUDA stream
+        handle `stream` (0: the legacy default stream); the codestream comes back as bytes, or goes to device memory
+        at out_ptr (capacity out_cap) and its length is returned"""
+        n = C.c_uint64()
+        if out_ptr is None:
+            self._check(self.L.ojb_enc_encode_device(self.h, C.byref(image), stream, self._out.ctypes.data, self._out.size,
+                                                     C.byref(n), 0))
+            return self._out[:n.value].tobytes()
+        self._check(self.L.ojb_enc_encode_device(self.h, C.byref(image), stream, out_ptr, out_cap, C.byref(n), 1))
+        return int(n.value)
+
+    def encode_tensor(self, t, layout="chw", stream=None, out=None):
+        """encode a frame that is a CUDA tensor (see _tensor_image for the shapes; dtype uint8 / uint16 / int32 as the
+        sample container) once the work queued on `stream` (default: torch's current stream) is done.  Returns the
+        codestream as a CUDA uint8 tensor, or, with `out` (a CUDA uint8 tensor), writes it there and returns its
+        length.  The codestream never leaves the device.  The returned tensor belongs to `stream`: work queued there
+        after the call sees it complete."""
+        import torch
+        img = _tensor_image(t, layout, self.sample_type, self.dims)
+        where = (t[0] if isinstance(t, (list, tuple)) else t).device
+        s = torch.cuda.current_stream(where) if stream is None else stream
+        if out is not None:
+            if not (out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous()):
+                raise ValueError("out is a contiguous CUDA uint8 tensor")
+            return self.encode_device(img, s.cuda_stream, out.data_ptr(), out.numel())
+        # one staging buffer per encoder: the same output address every call, so the frame's work replays as a graph.
+        # The copy out of it runs on `s`; the next call, whatever stream it names, writes the buffer only after that copy
+        dev = getattr(self, "_dev_out", None)
+        if dev is None or dev.device != where:
+            dev = self._dev_out = torch.empty(self._out.size, dtype=torch.uint8, device=where)
+        copied = getattr(self, "_copied", None)
+        if copied is not None:
+            s.wait_event(copied)
+        n = self.encode_device(img, s.cuda_stream, dev.data_ptr(), dev.numel())
+        with torch.cuda.stream(s):
+            res = torch.empty(n + 32, dtype=torch.uint8, device=where)     # 32 readable bytes past the end
+            res[:n].copy_(dev[:n])
+        self._copied = torch.cuda.Event()
+        self._copied.record(s)
+        return res[:n]
+
     def encode_lines(self, planes):
         """the reference's exchange() loop + flush()."""
         nc = C.c_uint32()
@@ -296,6 +379,55 @@ class Decoder(_Base):
         self._check(self.L.ojb_dec_read_headers_device(self.h, dev_ptr, length, sample_type, C.byref(fi)))
         self.info = fi
         return fi
+
+    def decode_device(self, image, stream=0):
+        """decode (after read_headers or read_headers_device) into device memory described by `image` (see
+        device_image), after the work queued on the CUDA stream handle `stream` (0: the legacy default stream)"""
+        self._check(self.L.ojb_dec_decode_device(self.h, C.byref(image), stream))
+
+    def decode_tensor(self, cs, out=None, layout="chw", stream=None, sample_type=None):
+        """decode a codestream -- bytes / ndarray in host memory, or a CUDA uint8 tensor, whose body then never leaves
+        the device (read_headers_device) -- into the CUDA tensor `out` (see _tensor_image for the shapes), or into a
+        new one: (C, H, W) / (H, W, C) when the components share a size, else a list of 2-D tensors.  The container
+        follows out's dtype, else sample_type (default I32).  Writing waits for the work queued on `stream` (default:
+        torch's current stream); the call returns with the samples in place."""
+        import torch
+        if sample_type is None:
+            sample_type = I32
+            if out is not None:
+                o = out[0] if isinstance(out, (list, tuple)) else out
+                sample_type = {torch.uint8: U8, torch.uint16: U16, torch.int32: I32}.get(o.dtype, I32)
+        if isinstance(cs, torch.Tensor):
+            if not (cs.is_cuda and cs.dtype == torch.uint8 and cs.dim() == 1 and cs.is_contiguous()):
+                raise ValueError("a codestream tensor is a contiguous 1-D CUDA uint8 tensor")
+            n = cs.numel()
+            if cs.untyped_storage().nbytes() - cs.storage_offset() - n < 32:      # the reader wants 32 bytes of slack
+                pad = torch.zeros(n + 32, dtype=torch.uint8, device=cs.device)
+                pad[:n].copy_(cs)
+                cs = pad[:n]
+            # the headers are read on the host: the bytes must be complete before the call
+            torch.cuda.current_stream(cs.device).synchronize()
+            if stream is not None:
+                stream.synchronize()
+            self._cs_keep = cs
+            self.read_headers_device(cs.data_ptr(), n, sample_type)
+        else:
+            self.read_headers(cs, sample_type)
+        fi = self.info
+        dims = [(fi.comp_w[c], fi.comp_h[c]) for c in range(fi.num_comps)]
+        s = torch.cuda.current_stream() if stream is None else stream
+        if out is None:                    # allocated on `s`, the stream the decoder's writes are ordered after
+            dt = getattr(torch, _TORCH_DTYPE[sample_type])
+            dev = cs.device if isinstance(cs, torch.Tensor) else torch.device("cuda", torch.cuda.current_device())
+            with torch.cuda.stream(s):
+                if len(set(dims)) == 1:
+                    w, h = dims[0]
+                    shape = (len(dims), h, w) if layout == "chw" else (h, w, len(dims))
+                    out = torch.empty(shape, dtype=dt, device=dev)
+                else:
+                    out = [torch.empty((h, w), dtype=dt, device=dev) for w, h in dims]
+        self.decode_device(_tensor_image(out, layout, sample_type, dims), s.cuda_stream)
+        return out
 
     @property
     def mirror_bytes(self):

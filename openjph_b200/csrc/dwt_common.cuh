@@ -49,6 +49,19 @@ __device__ __forceinline__ int reflect_coord(int u, int lo, int hi) {
 // the negative values, bias = 2^(B-1) + 1; an involution
 __device__ __forceinline__ int nlt_type3(int v, int bias) { return v >= 0 ? v : -v - bias; }
 
+__device__ __forceinline__ uint32_t src_esize(uint32_t src_type) { return src_type == SRC_U8 ? 1u : (src_type == SRC_U16 ? 2u : 4u); }
+
+// component slot k of a first-level job as the kernels address it: sample (u, v) of the resolution (relative to its
+// origin) at org + v * pitch + u * step, all in bytes
+struct ImgView { unsigned char* org; uint64_t pitch; uint32_t step, pad; };
+__device__ __forceinline__ ImgView img_view(const ImgComp* img, const DwtJob& J, uint32_t k) {
+  const ImgComp c = img[J.img_comp[k]];
+  ImgView w;
+  w.step = c.col * src_esize(J.src_type); w.pitch = c.pitch; w.pad = 0;
+  w.org = reinterpret_cast<unsigned char*>(c.base) + (size_t)J.img_y[k] * c.pitch + (size_t)J.img_x[k] * w.step;
+  return w;
+}
+
 // locate the job a CTA belongs to (jobs sorted by cta_base)
 __device__ __forceinline__ uint32_t find_job(const DwtJob* jobs, uint32_t njobs, uint32_t cta) {
   uint32_t lo = 0, hi = njobs;

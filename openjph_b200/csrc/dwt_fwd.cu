@@ -28,11 +28,10 @@ template <> struct Px<true, false>  { typedef int T; typedef int I; };
 template <> struct Px<false, false> { typedef float T; typedef int I; };
 template <> struct Px<true, true>   { typedef long long T; typedef long long I; };
 
-__device__ __forceinline__ int load_sample(const void* img, uint32_t type, uint64_t byte_off, size_t idx) {
-  const unsigned char* base = reinterpret_cast<const unsigned char*>(img) + byte_off;
-  if (type == SRC_U8) return (int)base[idx];
-  if (type == SRC_U16) return (int)reinterpret_cast<const unsigned short*>(base)[idx];
-  return reinterpret_cast<const int*>(base)[idx];
+__device__ __forceinline__ int load_sample(const unsigned char* p, uint32_t type) {
+  if (type == SRC_U8) return (int)*p;
+  if (type == SRC_U16) return (int)*reinterpret_cast<const unsigned short*>(p);
+  return *reinterpret_cast<const int*>(p);
 }
 
 // 9/7: dst += coeff * (a + b), separate multiply and add (no FMA), ojph_transform.cpp:703
@@ -42,19 +41,22 @@ __device__ __forceinline__ float irv_step(float d, float a, float b, float c) {
 
 template <bool REV, bool WIDE>
 __global__ void __launch_bounds__(DW_THREADS)
-dwt_fwd_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const void* __restrict__ image,
+dwt_fwd_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const ImgComp* __restrict__ img,
                uint32_t* __restrict__ coef)
 {
   typedef typename Px<REV, WIDE>::T T;
   typedef typename Px<REV, WIDE>::I I;
   OJB_DYN_SMEM(T, smem);
   __shared__ DwtJob sj;
+  __shared__ ImgView sv[3];
   {
     uint32_t ji = find_job(jobs, njobs, blockIdx.x);
     const uint32_t* s = reinterpret_cast<const uint32_t*>(&jobs[ji]);
     uint32_t* d = reinterpret_cast<uint32_t*>(&sj);
     for (uint32_t i = threadIdx.x; i < sizeof(DwtJob) / 4; i += blockDim.x) d[i] = s[i];
   }
+  __syncthreads();
+  if (sj.first && threadIdx.x < sj.ncomp) sv[threadIdx.x] = img_view(img, sj, threadIdx.x);
   __syncthreads();
   const DwtJob& J = sj;
   const uint32_t tid = threadIdx.x;
@@ -73,31 +75,30 @@ dwt_fwd_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const void* __re
     T val[3];
     if (J.first) {
       I iv[3];
-      for (uint32_t k = 0; k < nc; ++k)
-        iv[k] = (I)load_sample(image, J.src_type, J.full_off[k],
-                               (size_t)(v - y0) * J.full_stride[k] + (size_t)(u - x0));
+      for (uint32_t k = 0; k < 3; ++k) if (k < nc)
+        iv[k] = (I)load_sample(sv[k].org + (size_t)(v - y0) * sv[k].pitch + (size_t)(u - x0) * sv[k].step, J.src_type);
       if (J.nlt_mask) {
         const I bias = ((I)1 << (J.bit_depth - 1)) + 1;
-        for (uint32_t k = 0; k < nc; ++k) if ((J.nlt_mask >> k) & 1u) iv[k] = iv[k] >= 0 ? iv[k] : -iv[k] - bias;
+        for (uint32_t k = 0; k < 3; ++k) if (k < nc) if ((J.nlt_mask >> k) & 1u) iv[k] = iv[k] >= 0 ? iv[k] : -iv[k] - bias;
       }
       if (REV) {
         const I shift = J.is_signed ? (I)0 : ((I)1 << (J.bit_depth - 1));
-        for (uint32_t k = 0; k < nc; ++k) iv[k] -= shift;
+        for (uint32_t k = 0; k < 3; ++k) if (k < nc) iv[k] -= shift;
         // with the colour transform the reference converts into 32-bit temporary lines whatever the precision
         // (tile::pre_alloc / finalize_alloc, ojph_tile.cpp:181-183, :312-317): the level-shifted samples wrap to
         // si32 before the (64-bit) RCT -- byte-identical streams for 32-bit samples need the same
         if (WIDE && nc == 3)
-          for (uint32_t k = 0; k < nc; ++k) iv[k] = (I)(int)iv[k];
+          for (uint32_t k = 0; k < 3; ++k) if (k < nc) iv[k] = (I)(int)iv[k];
         if (nc == 3) {   // RCT
           I rr = iv[0], gg = iv[1], bb = iv[2];
           iv[0] = (rr + (gg << 1) + bb) >> 2; iv[1] = bb - gg; iv[2] = rr - gg;
         }
-        for (uint32_t k = 0; k < nc; ++k) val[k] = (T)iv[k];
+        for (uint32_t k = 0; k < 3; ++k) if (k < nc) val[k] = (T)iv[k];
       } else {
         const float mul = (float)(1.0 / (double)(1ull << J.bit_depth));
         const int half = J.is_signed ? 0 : (1 << (J.bit_depth - 1));
         float f[3];
-        for (uint32_t k = 0; k < nc; ++k) f[k] = __fmul_rn((float)((int)iv[k] - half), mul);
+        for (uint32_t k = 0; k < 3; ++k) if (k < nc) f[k] = __fmul_rn((float)((int)iv[k] - half), mul);
         if (nc == 3) {   // ICT
           float rr = f[0], gg = f[1], bb = f[2];
           float yy = __fadd_rn(__fadd_rn(__fmul_rn(ICT_ALPHA_RF, rr), __fmul_rn(ICT_ALPHA_GF, gg)),
@@ -106,13 +107,13 @@ dwt_fwd_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const void* __re
           f[1] = __fmul_rn(ICT_BETA_CBF, __fsub_rn(bb, yy));
           f[2] = __fmul_rn(ICT_BETA_CRF, __fsub_rn(rr, yy));
         }
-        for (uint32_t k = 0; k < nc; ++k) val[k] = (T)f[k];
+        for (uint32_t k = 0; k < 3; ++k) if (k < nc) val[k] = (T)f[k];
       }
     } else {
       const T* src = reinterpret_cast<const T*>(coef) + J.full_off[0];
       val[0] = src[(size_t)(v - y0) * J.full_stride[0] + (size_t)(u - x0)];
     }
-    for (uint32_t k = 0; k < nc; ++k) smem[k * DW_TILE_WORDS + r * DW_PITCH + c] = val[k];
+    for (uint32_t k = 0; k < 3; ++k) if (k < nc) smem[k * DW_TILE_WORDS + r * DW_PITCH + c] = val[k];
   }
   __syncthreads();
 
@@ -242,22 +243,22 @@ void dwt_tiling(uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, uint32_t& tx, 
 }
 
 void launch_dwt_fwd(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                    uint32_t max_ncomp, const void* image, uint32_t* coef, cudaStream_t st, bool wide)
+                    uint32_t max_ncomp, const ImgComp* img, uint32_t* coef, cudaStream_t st, bool wide)
 {
   if (total_ctas == 0) return;
   size_t smem = (size_t)max_ncomp * DW_TILE_WORDS * (wide ? 8 : 4);
   if (reversible && wide) {
     auto k = dwt_fwd_kernel<true, true>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, image, coef);
+    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, img, coef);
   } else if (reversible) {
     auto k = dwt_fwd_kernel<true, false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, image, coef);
+    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, img, coef);
   } else {
     auto k = dwt_fwd_kernel<false, false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, image, coef);
+    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, img, coef);
   }
 }
 

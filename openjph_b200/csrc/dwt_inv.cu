@@ -22,11 +22,10 @@ template <> struct PxI<false, false> { typedef float T; typedef int I; };
 template <> struct PxI<true, true>   { typedef long long T; typedef long long I; };      // 64-bit lines (precision > 32 bits)
 
 // 8 / 16-bit containers clamp to the component's range [0, smax] as the reference's file writers do
-__device__ __forceinline__ void store_sample(void* img, uint32_t type, uint64_t byte_off, size_t idx, int v, int smax) {
-  unsigned char* base = reinterpret_cast<unsigned char*>(img) + byte_off;
-  if (type == SRC_U8) base[idx] = (unsigned char)min(max(v, 0), smax);
-  else if (type == SRC_U16) reinterpret_cast<unsigned short*>(base)[idx] = (unsigned short)min(max(v, 0), smax);
-  else reinterpret_cast<int*>(base)[idx] = v;
+__device__ __forceinline__ void store_sample(unsigned char* p, uint32_t type, int v, int smax) {
+  if (type == SRC_U8) *p = (unsigned char)min(max(v, 0), smax);
+  else if (type == SRC_U16) *reinterpret_cast<unsigned short*>(p) = (unsigned short)min(max(v, 0), smax);
+  else *reinterpret_cast<int*>(p) = v;
 }
 
 // float -> integer as the reference's SIMD builds do it (cvtps: round to nearest, ties to even;
@@ -36,19 +35,22 @@ __device__ __forceinline__ int round_haz(float t) { return __float2int_rn(t); }
 
 template <bool REV, bool WIDE>
 __global__ void __launch_bounds__(DW_THREADS)
-dwt_inv_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, void* __restrict__ image,
+dwt_inv_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const ImgComp* __restrict__ img,
                uint32_t* __restrict__ coef)
 {
   typedef typename PxI<REV, WIDE>::T T;
   typedef typename PxI<REV, WIDE>::I I;
   OJB_DYN_SMEM(T, smem);
   __shared__ DwtJob sj;
+  __shared__ ImgView sv[3];
   {
     uint32_t ji = find_job(jobs, njobs, blockIdx.x);
     const uint32_t* s = reinterpret_cast<const uint32_t*>(&jobs[ji]);
     uint32_t* d = reinterpret_cast<uint32_t*>(&sj);
     for (uint32_t i = threadIdx.x; i < sizeof(DwtJob) / 4; i += blockDim.x) d[i] = s[i];
   }
+  __syncthreads();
+  if (sj.first && threadIdx.x < sj.ncomp) sv[threadIdx.x] = img_view(img, sj, threadIdx.x);
   __syncthreads();
   const DwtJob& J = sj;
   const uint32_t tid = threadIdx.x;
@@ -227,29 +229,30 @@ dwt_inv_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, void* __restrict
       for (uint32_t k = 0; k < nc; ++k) if ((J.nlt_mask >> k) & 1u) out[k] = nlt_type3(out[k], bias);
     }
     for (uint32_t k = 0; k < nc; ++k)
-      store_sample(image, J.src_type, J.full_off[k], (size_t)(v - y0) * J.full_stride[k] + (size_t)(u - x0), out[k], (int)((1u << (J.bit_depth & 31u)) - 1u));
+      store_sample(sv[k].org + (size_t)(v - y0) * sv[k].pitch + (size_t)(u - x0) * sv[k].step, J.src_type, out[k],
+                   (int)((1u << (J.bit_depth & 31u)) - 1u));
   }
 }
 
 } // namespace
 
 void launch_dwt_inv(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                    uint32_t max_ncomp, void* image, uint32_t* coef, cudaStream_t st, bool wide)
+                    uint32_t max_ncomp, const ImgComp* img, uint32_t* coef, cudaStream_t st, bool wide)
 {
   if (total_ctas == 0) return;
   size_t smem = (size_t)max_ncomp * DW_TILE_WORDS * (wide ? 8 : 4);
   if (reversible && wide) {
     auto k = dwt_inv_kernel<true, true>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, image, coef);
+    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, img, coef);
   } else if (reversible) {
     auto k = dwt_inv_kernel<true, false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, image, coef);
+    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, img, coef);
   } else {
     auto k = dwt_inv_kernel<false, false>;
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, image, coef);
+    OJB_LAUNCH(k, dim3(total_ctas), dim3(DW_THREADS), smem, st, jobs, njobs, img, coef);
   }
 }
 

@@ -147,34 +147,35 @@ __device__ __forceinline__ bool strip_setup(const DwtJob& J, uint32_t strip, uin
 // in flight) and later reads back exactly the bytes it requested, so no cross-lane synchronisation
 // is needed -- cp.async.wait_group orders a lane's own copies.
 
-// The image buffer and the coefficient arena are addressed with 32-bit byte offsets from their
-// (256-byte aligned) base; alignment is tested on the offset.
-// request four 32-bit elements base[row + c[0..3]] into a 16-byte slot (offsets in bytes)
-__device__ __forceinline__ void issue4_w(unsigned char* d, const unsigned char* base, uint32_t row_off, const StripGeom& g) {
-  const uint32_t o = row_off + 4u * (uint32_t)g.c[0];
-  if (g.interior && (o & 15u) == 0) cp_async<16>(d, base + o);
+// A row is addressed as a pointer plus 32-bit byte offsets (column c at row + c * step); alignment is tested on
+// the address itself.  step is the element size where the columns are contiguous (the coefficient arena, planar
+// image rows), a multiple of it for interleaved image rows, which take the per-sample requests.
+// request four 32-bit elements row[c[0..3]] into a 16-byte slot
+__device__ __forceinline__ void issue4_w(unsigned char* d, const unsigned char* row, uint32_t step, const StripGeom& g) {
+  const unsigned char* p = row + step * (uint32_t)g.c[0];
+  if (g.interior && step == 4u && ((uint32_t)(size_t)p & 15u) == 0) cp_async<16>(d, p);
   else {
     #pragma unroll
-    for (int i = 0; i < 4; ++i) cp_async<4>(d + 4 * i, base + row_off + 4u * (uint32_t)g.c[i]);
+    for (int i = 0; i < 4; ++i) cp_async<4>(d + 4 * i, row + step * (uint32_t)g.c[i]);
   }
 }
-__device__ __forceinline__ void issue4_u16(unsigned char* d, const unsigned char* base, uint32_t row_off, const StripGeom& g) {
-  const uint32_t o = row_off + 2u * (uint32_t)g.c[0];
-  if (g.interior && (o & 7u) == 0) cp_async<8>(d, base + o);
-  else if (g.interior && (o & 3u) == 0) { cp_async<4>(d, base + o); cp_async<4>(d + 4, base + o + 4); }
-  else {                                   // mirrored or odd-aligned columns: plain loads (edge lanes)
+__device__ __forceinline__ void issue4_u16(unsigned char* d, const unsigned char* row, uint32_t step, const StripGeom& g) {
+  const unsigned char* p = row + step * (uint32_t)g.c[0];
+  const uint32_t a = (uint32_t)(size_t)p;
+  if (g.interior && step == 2u && (a & 7u) == 0) cp_async<8>(d, p);
+  else if (g.interior && step == 2u && (a & 3u) == 0) { cp_async<4>(d, p); cp_async<4>(d + 4, p + 4); }
+  else {                                   // mirrored, odd-aligned or interleaved columns: plain loads
     unsigned short* ds = reinterpret_cast<unsigned short*>(d);
-    const unsigned short* p = reinterpret_cast<const unsigned short*>(base + row_off);
     #pragma unroll
-    for (int i = 0; i < 4; ++i) ds[i] = p[g.c[i]];
+    for (int i = 0; i < 4; ++i) ds[i] = *reinterpret_cast<const unsigned short*>(row + step * (uint32_t)g.c[i]);
   }
 }
-__device__ __forceinline__ void issue4_u8(unsigned char* d, const unsigned char* base, uint32_t row_off, const StripGeom& g) {
-  const uint32_t o = row_off + (uint32_t)g.c[0];
-  if (g.interior && (o & 3u) == 0) cp_async<4>(d, base + o);
+__device__ __forceinline__ void issue4_u8(unsigned char* d, const unsigned char* row, uint32_t step, const StripGeom& g) {
+  const unsigned char* p = row + step * (uint32_t)g.c[0];
+  if (g.interior && step == 1u && ((uint32_t)(size_t)p & 3u) == 0) cp_async<4>(d, p);
   else {
     #pragma unroll
-    for (int i = 0; i < 4; ++i) d[i] = base[row_off + (uint32_t)g.c[i]];
+    for (int i = 0; i < 4; ++i) d[i] = row[step * (uint32_t)g.c[i]];
   }
 }
 // two consecutive 32-bit words
@@ -193,14 +194,15 @@ template <typename T> __device__ __forceinline__ T from_bits(uint32_t v) { T r; 
 // strip that does not touch the left / right edge when offsets and strides are even enough, i.e. almost
 // always; the per-request tests above otherwise get if-converted and both variants are issued every time.)
 template <int NC, int SRC>
-__device__ __forceinline__ bool strip_fast_fwd(const DwtJob& J, const StripGeom& g) {
+__device__ __forceinline__ bool strip_fast_fwd(const DwtJob& J, const ImgView* V, const StripGeom& g) {
   constexpr bool FIRST = SRC != SRC_COEF;
   constexpr uint32_t ES = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
   bool ok = g.interior;
   #pragma unroll
   for (int k = 0; k < (FIRST ? NC : 1); ++k) {
-    const uint32_t off = FIRST ? (uint32_t)J.full_off[k] : (uint32_t)J.full_off[0] * 4u;
-    ok = ok && ((off + (uint32_t)g.c[0] * ES) % (4u * ES)) == 0 && ((J.full_stride[k] * ES) % (4u * ES)) == 0;
+    const uint32_t off = FIRST ? (uint32_t)(size_t)V[k].org : (uint32_t)J.full_off[0] * 4u;
+    const uint32_t pitch = FIRST ? (uint32_t)V[k].pitch : J.full_stride[0] * ES;
+    ok = ok && (!FIRST || V[k].step == ES) && ((off + (uint32_t)g.c[0] * ES) % (4u * ES)) == 0 && (pitch % (4u * ES)) == 0;
   }
   return __all_sync(0xFFFFFFFFu, ok);
 }
@@ -228,44 +230,127 @@ __device__ __forceinline__ bool strip_fast_inv(const DwtJob& J, const StripGeom&
   return __all_sync(0xFFFFFFFFu, ok);
 }
 
+// ---- interleaved first level (ILV variant): the three components of a colour-transform job sit next to each other
+// in memory, S = 3 or 4 samples per pixel (RGB / RGBA).  A lane's four pixels are then 4 S contiguous samples: they
+// travel as S whole requests of 4 ES bytes each (12 / 24 / 48 or 16 / 32 / 64 bytes per row) and sit in the lane's
+// FIFO slot (16 ES bytes) exactly as in memory.  Warp-uniform gate as strip_fast_*: every lane interior, the first
+// pixel of every lane and the pitch multiples of 4 ES bytes.
+template <int SRC>
+__device__ __forceinline__ bool strip_fast_ilv(const ImgView* V, const StripGeom& g, uint32_t S) {
+  constexpr uint32_t ES = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
+  const uint32_t a = (uint32_t)(size_t)V[0].org + (uint32_t)g.c[0] * S * ES;
+  return __all_sync(0xFFFFFFFFu, g.interior && (a % (4u * ES)) == 0 && ((uint32_t)V[0].pitch % (4u * ES)) == 0);
+}
+template <int SRC>
+__device__ __forceinline__ void ilv_issue_row(const StripGeom& g, const ImgView* V, int vr, unsigned char* st, uint32_t S) {
+  constexpr uint32_t ES = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
+  if (g.fast) {
+    const unsigned char* p = V[0].org + ((uint32_t)vr * (uint32_t)V[0].pitch + (uint32_t)g.c[0] * S * ES);
+    #pragma unroll
+    for (int j = 0; j < 3; ++j) cp_async<4 * ES>(st + j * 4 * ES, p + j * 4 * ES);
+    if (S == 4) cp_async<4 * ES>(st + 12 * ES, p + 12 * ES);
+    return;
+  }
+  #pragma unroll
+  for (int k = 0; k < 3; ++k) {              // edge lanes (mirrored columns) or misaligned rows: plain loads
+    const unsigned char* row = V[k].org + (uint32_t)vr * (uint32_t)V[k].pitch;
+    #pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const unsigned char* q = row + (uint32_t)g.c[i] * V[k].step;
+      unsigned char* d = st + ((uint32_t)i * S + (uint32_t)k) * ES;
+      if (ES == 1) *d = *q;
+      else if (ES == 2) *reinterpret_cast<unsigned short*>(d) = *reinterpret_cast<const unsigned short*>(q);
+      else *reinterpret_cast<uint32_t*>(d) = *reinterpret_cast<const uint32_t*>(q);
+    }
+  }
+}
+// sample (pixel i, component k) of the 4 S samples at d (4-byte aligned)
+template <int S, uint32_t ES>
+__device__ __forceinline__ void ilv_unpack(const unsigned char* d, int (&iv)[3][4]) {
+  uint32_t w[S * ES];
+  #pragma unroll
+  for (int j = 0; j < (int)(S * ES); ++j) w[j] = reinterpret_cast<const uint32_t*>(d)[j];
+  #pragma unroll
+  for (int i = 0; i < 4; ++i)
+    #pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const int n = i * S + k;
+      iv[k][i] = ES == 1 ? (int)((w[n >> 2] >> (8 * (n & 3))) & 0xFFu)
+               : ES == 2 ? (int)((w[n >> 1] >> (16 * (n & 1))) & 0xFFFFu) : (int)w[n];
+    }
+}
+// the three components of four pixels (container values) to memory at p (4 ES-byte aligned): S = 3, three whole
+// vectors of 4 ES bytes; S = 4, per pixel one vector for the first two components and one for the third, so the
+// fourth sample of each pixel (a channel the codec does not code) is left as it is
+template <int S, uint32_t ES>
+__device__ __forceinline__ void ilv_store(unsigned char* p, const uint32_t (&q)[3][4]) {
+  if (S == 3) {
+    uint32_t w[3 * ES];
+    #pragma unroll
+    for (int j = 0; j < (int)(3 * ES); ++j) w[j] = 0;
+    #pragma unroll
+    for (int i = 0; i < 4; ++i)
+      #pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const int n = i * 3 + k;
+        if (ES == 1) w[n >> 2] |= q[k][i] << (8 * (n & 3));
+        else if (ES == 2) w[n >> 1] |= q[k][i] << (16 * (n & 1));
+        else w[n] = q[k][i];
+      }
+    #pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      if (ES == 1) reinterpret_cast<uint32_t*>(p)[j] = w[j];
+      else if (ES == 2) reinterpret_cast<uint2*>(p)[j] = make_uint2(w[2 * j], w[2 * j + 1]);
+      else reinterpret_cast<uint4*>(p)[j] = make_uint4(w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
+    }
+  } else {
+    #pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      unsigned char* px = p + i * 4 * ES;
+      if (ES == 1) { *reinterpret_cast<unsigned short*>(px) = (unsigned short)(q[0][i] | (q[1][i] << 8)); px[2] = (unsigned char)q[2][i]; }
+      else if (ES == 2) { *reinterpret_cast<uint32_t*>(px) = q[0][i] | (q[1][i] << 16); *reinterpret_cast<unsigned short*>(px + 4) = (unsigned short)q[2][i]; }
+      else { *reinterpret_cast<uint2*>(px) = make_uint2(q[0][i], q[1][i]); *reinterpret_cast<uint32_t*>(px + 8) = q[2][i]; }
+    }
+  }
+}
+
 // ---- forward ---------------------------------------------------------------------------------
-// request source row v (mirrored into the resolution) into the row slot `st` (lane offset included)
-template <int NC, int SRC>
-__device__ __forceinline__ void fwd_issue_row(const DwtJob& J, const StripGeom& g, const void* image,
+// request source row v (mirrored into the resolution) into the row slot `st` (lane offset included); cpitch = bytes
+// between the components' slots, or (ILV) samples per pixel
+template <int NC, int SRC, bool ILV>
+__device__ __forceinline__ void fwd_issue_row(const DwtJob& J, const StripGeom& g, const ImgView* V,
                                               const uint32_t* coef, int v, unsigned char* st, uint32_t cpitch)
 {
   constexpr bool FIRST = SRC != SRC_COEF;     // the full-resolution side is the image
+  constexpr uint32_t ES = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
   const int vr = reflect_coord(v, g.y0, g.y1 - 1) - g.y0;
+  if constexpr (ILV) { ilv_issue_row<SRC>(g, V, vr, st, cpitch); return; }
   if (g.fast) {                               // one aligned vector per component, no per-request tests
-    constexpr uint32_t ES = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
-    const unsigned char* base = FIRST ? reinterpret_cast<const unsigned char*>(image) : reinterpret_cast<const unsigned char*>(coef);
     #pragma unroll
     for (int k = 0; k < (FIRST ? NC : 1); ++k) {
-      const uint32_t o = (FIRST ? (uint32_t)J.full_off[k] : (uint32_t)J.full_off[0] * 4u) +
-                         ((uint32_t)vr * J.full_stride[k] + (uint32_t)g.c[0]) * ES;
-      cp_async<4 * ES>(st + (size_t)k * cpitch, base + o);
+      const unsigned char* p = FIRST
+        ? V[k].org + ((uint32_t)vr * (uint32_t)V[k].pitch + (uint32_t)g.c[0] * ES)
+        : reinterpret_cast<const unsigned char*>(coef) + ((uint32_t)J.full_off[0] * 4u + ((uint32_t)vr * J.full_stride[0] + (uint32_t)g.c[0]) * ES);
+      cp_async<4 * ES>(st + (size_t)k * cpitch, p);
     }
     return;
   }
   if (FIRST) {
-    const unsigned char* base = reinterpret_cast<const unsigned char*>(image);
     #pragma unroll
     for (int k = 0; k < NC; ++k) {
-      constexpr uint32_t ES = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
-      const uint32_t row_off = (uint32_t)J.full_off[k] + (uint32_t)vr * J.full_stride[k] * ES;     // bytes
+      const unsigned char* row = V[k].org + (uint32_t)vr * (uint32_t)V[k].pitch;
       unsigned char* d = st + (size_t)k * cpitch;
-      if (SRC == SRC_U16) issue4_u16(d, base, row_off, g);
-      else if (SRC == SRC_U8) issue4_u8(d, base, row_off, g);
-      else issue4_w(d, base, row_off, g);
+      if (SRC == SRC_U16) issue4_u16(d, row, V[k].step, g);
+      else if (SRC == SRC_U8) issue4_u8(d, row, V[k].step, g);
+      else issue4_w(d, row, V[k].step, g);
     }
   } else {
-    issue4_w(st, reinterpret_cast<const unsigned char*>(coef),
-             ((uint32_t)J.full_off[0] + (uint32_t)vr * J.full_stride[0]) * 4u, g);
+    issue4_w(st, reinterpret_cast<const unsigned char*>(coef) + ((uint32_t)J.full_off[0] + (uint32_t)vr * J.full_stride[0]) * 4u, 4u, g);
   }
 }
 
 // read a row slot back: level shift / int->float and RCT / ICT at level 1
-template <bool REV, int NC, int SRC>
+template <bool REV, int NC, int SRC, bool ILV>
 __device__ __forceinline__ void fwd_read_row(const DwtJob& J, const unsigned char* st, uint32_t cpitch,
                                              typename Tp<REV>::T (&a)[NC][4])
 {
@@ -273,6 +358,10 @@ __device__ __forceinline__ void fwd_read_row(const DwtJob& J, const unsigned cha
   typedef typename Tp<REV>::T T;
   if (FIRST) {
     int iv[NC][4];
+    if constexpr (ILV) {
+      constexpr uint32_t ES = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
+      if (cpitch == 3) ilv_unpack<3, ES>(st, iv); else ilv_unpack<4, ES>(st, iv);
+    } else {
     #pragma unroll
     for (int k = 0; k < NC; ++k) {
       const unsigned char* d = st + (size_t)k * cpitch;
@@ -286,6 +375,7 @@ __device__ __forceinline__ void fwd_read_row(const DwtJob& J, const unsigned cha
         const uint4 t = *reinterpret_cast<const uint4*>(d);
         iv[k][0] = (int)t.x; iv[k][1] = (int)t.y; iv[k][2] = (int)t.z; iv[k][3] = (int)t.w;
       }
+    }
     }
     if (J.nlt_mask) {
       const int bias = (1 << (J.bit_depth - 1)) + 1;
@@ -382,13 +472,16 @@ __device__ __forceinline__ void fwd_store_pair(const DwtJob& J, const StripGeom&
 // interior strip of the usual geometries) are requested by ONE lane with cp.async.bulk (SASS UBLKCP) -- one copy per
 // component row into a row slot of 32 x slot + 16 bytes -- and awaited on an mbarrier per FIFO stage, instead of one
 // cp.async (LDGSTS) per lane; edge strips keep the per-lane requests.  Selected by the host (OJB_DWT_TMA).
-template <bool REV, int NC, int SRC, bool TMA>
+// ILV: the interleaved layout variant (see ilv_issue_row), colour-transform jobs only
+template <bool REV, int NC, int SRC, bool TMA, bool ILV>
 __global__ void __launch_bounds__(DS_WARPS * 32, (REV || NC == 1) ? 5 : 3)
-dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const void* __restrict__ image,
+dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const ImgComp* __restrict__ img,
                       uint32_t* __restrict__ coef)
 {
   typedef typename Tp<REV>::T T;
+  constexpr bool FIRSTK = SRC != SRC_COEF;
   __shared__ DwtJob sj;
+  __shared__ ImgView sv[FIRSTK ? NC : 1];
   __shared__ unsigned long long s_bar[TMA ? DS_WARPS * DS_STAGES : 1];
   {
     uint32_t ji = find_job(jobs, njobs, blockIdx.x);
@@ -397,7 +490,12 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
     for (uint32_t i = threadIdx.x; i < sizeof(DwtJob) / 4; i += blockDim.x) d[i] = s[i];
   }
   __syncthreads();
+  if (FIRSTK) {
+    if (threadIdx.x < NC) sv[threadIdx.x] = img_view(img, sj, threadIdx.x);
+    __syncthreads();
+  }
   const DwtJob& J = sj;
+  const ImgView* V = sv;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // CTA = DS_WARPS adjacent strips of one row chunk
   const uint32_t cta = blockIdx.x - J.cta_base;
@@ -406,13 +504,14 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
   if (strip >= J.tiles_x) return;
   StripGeom g;
   if (!strip_setup(J, strip, chunk, lane, g)) return;
-  g.fast = strip_fast_fwd<NC, SRC>(J, g);
+  constexpr uint32_t ESK = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
+  const uint32_t S = ILV ? V[0].step / ESK : 0u;                       // ILV: samples per pixel
+  g.fast = ILV ? strip_fast_ilv<SRC>(V, g, S) : strip_fast_fwd<NC, SRC>(J, V, g);
 
   // the lane's FIFO: DS_STAGES stages of one row pair each
   OJB_DYN_SMEM(unsigned char, s_ring);
-  const uint32_t slot = (SRC == SRC_U8 || SRC == SRC_U16) ? 8u : 16u;   // 4 samples in their container
-  constexpr bool FIRSTK = SRC != SRC_COEF;
-  constexpr uint32_t ESK = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
+  // 4 samples in their container (ILV: 4 pixels of up to 4 samples)
+  const uint32_t slot = ILV ? 16u * ESK : ((SRC == SRC_U8 || SRC == SRC_U16) ? 8u : 16u);
   // bulk-copy mode of this strip (warp-uniform): every row of every component starts at the same offset modulo 16
   bool tma = false;
   uint32_t skip = 0, c0l0 = 0;
@@ -421,14 +520,16 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
     bool ok = g.fast;
     #pragma unroll
     for (int k = 0; k < (FIRSTK ? NC : 1); ++k) {
-      const uint32_t off = (FIRSTK ? (uint32_t)J.full_off[k] : (uint32_t)J.full_off[0] * 4u) + c0l0 * ESK;
+      const uint32_t off = (FIRSTK ? (uint32_t)(size_t)V[k].org : (uint32_t)J.full_off[0] * 4u) + c0l0 * ESK;
+      const uint32_t pitch = FIRSTK ? (uint32_t)V[k].pitch : J.full_stride[0] * ESK;
       if (k == 0) skip = off & 15u;
-      ok = ok && (off & 15u) == skip && ((J.full_stride[k] * ESK) & 15u) == 0;
+      ok = ok && (off & 15u) == skip && (pitch & 15u) == 0;
     }
     tma = ok;
   }
-  const uint32_t cpitch = TMA ? 32 * slot + 16 : 32 * slot;            // bytes between the components of a row slot
-  const uint32_t row_bytes = NC * cpitch, stage_bytes = 2 * row_bytes;
+  // bytes between the components of a row slot (ILV: samples per pixel, one slot holds them all)
+  const uint32_t cpitch = ILV ? S : (TMA ? 32 * slot + 16 : 32 * slot);
+  const uint32_t row_bytes = ILV ? 32 * slot : NC * cpitch, stage_bytes = 2 * row_bytes;
   unsigned char* wring = s_ring + (size_t)warp * DS_STAGES * stage_bytes;
   unsigned char* ring = wring + (size_t)lane * slot + (tma ? skip : 0u);
   unsigned long long* bar = s_bar + (TMA ? warp * DS_STAGES : 0);
@@ -444,14 +545,15 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
       fence_proxy_async();
       const uint32_t nbytes = 32 * slot + 16;
       mbar_expect_tx(bar + stg, 2u * (FIRSTK ? NC : 1) * nbytes);
-      const unsigned char* base = FIRSTK ? reinterpret_cast<const unsigned char*>(image) : reinterpret_cast<const unsigned char*>(coef);
       #pragma unroll
       for (int r = 0; r < 2; ++r) {
         const int vr = reflect_coord(2 * kk - 1 + r, g.y0, g.y1 - 1) - g.y0;
         #pragma unroll
         for (int k = 0; k < (FIRSTK ? NC : 1); ++k) {
-          const uint32_t o = (FIRSTK ? (uint32_t)J.full_off[k] : (uint32_t)J.full_off[0] * 4u) + ((uint32_t)vr * J.full_stride[k] + c0l0) * ESK - skip;
-          bulk_g2s(wring + (size_t)stg * stage_bytes + (size_t)r * row_bytes + (size_t)k * cpitch, base + o, nbytes, bar + stg);
+          const unsigned char* p = FIRSTK
+            ? V[k].org + ((uint32_t)vr * (uint32_t)V[k].pitch + c0l0 * ESK - skip)
+            : reinterpret_cast<const unsigned char*>(coef) + ((uint32_t)J.full_off[0] * 4u + ((uint32_t)vr * J.full_stride[0] + c0l0) * ESK - skip);
+          bulk_g2s(wring + (size_t)stg * stage_bytes + (size_t)r * row_bytes + (size_t)k * cpitch, p, nbytes, bar + stg);
         }
       }
     }
@@ -463,9 +565,9 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
   T xe[NC][4];                                                // x[2k-2]
   {                                                           // priming row through the last stage
     unsigned char* sp = ring + (size_t)(DS_STAGES - 1) * stage_bytes;
-    fwd_issue_row<NC, SRC>(J, g, image, coef, 2 * k0 - 2, sp - (tma ? skip : 0u), cpitch);     // (per-lane request, old lane layout)
+    fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * k0 - 2, sp - (tma ? skip : 0u), cpitch);     // (per-lane request, old lane layout)
     cp_commit(); cp_wait<0>();
-    fwd_read_row<REV, NC, SRC>(J, sp - (tma ? skip : 0u), cpitch, xe);
+    fwd_read_row<REV, NC, SRC, ILV>(J, sp - (tma ? skip : 0u), cpitch, xe);
   }
   int issued = k0;
   #pragma unroll
@@ -474,8 +576,8 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
       if (TMA && tma) issue_tma(issued, (uint32_t)((issued - k0) % DS_STAGES));
       else {
         unsigned char* st = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
-        fwd_issue_row<NC, SRC>(J, g, image, coef, 2 * issued - 1, st, cpitch);
-        fwd_issue_row<NC, SRC>(J, g, image, coef, 2 * issued, st + row_bytes, cpitch);
+        fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, st, cpitch);
+        fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, st + row_bytes, cpitch);
       }
     }
     cp_commit(); ++issued;
@@ -492,8 +594,8 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
       if (TMA && tma) mbar_wait(bar + (k - k0) % DS_STAGES, (uint32_t)(((k - k0) / DS_STAGES) & 1));
       else cp_wait<DS_STAGES - 2>();
       const unsigned char* st = ring + (size_t)((k - k0) % DS_STAGES) * stage_bytes;
-      fwd_read_row<REV, NC, SRC>(J, st, cpitch, xo);
-      fwd_read_row<REV, NC, SRC>(J, st + row_bytes, cpitch, xn);
+      fwd_read_row<REV, NC, SRC, ILV>(J, st, cpitch, xo);
+      fwd_read_row<REV, NC, SRC, ILV>(J, st + row_bytes, cpitch, xn);
       #pragma unroll
       for (int c = 0; c < NC; ++c)
         #pragma unroll
@@ -507,8 +609,8 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
         if (TMA && tma) issue_tma(issued, (uint32_t)((issued - k0) % DS_STAGES));
         else {
           unsigned char* sn = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
-          fwd_issue_row<NC, SRC>(J, g, image, coef, 2 * issued - 1, sn, cpitch);
-          fwd_issue_row<NC, SRC>(J, g, image, coef, 2 * issued, sn + row_bytes, cpitch);
+          fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, sn, cpitch);
+          fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, sn + row_bytes, cpitch);
         }
       }
       cp_commit(); ++issued;
@@ -526,8 +628,8 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
       if (TMA && tma) mbar_wait(bar + (k - k0) % DS_STAGES, (uint32_t)(((k - k0) / DS_STAGES) & 1));
       else cp_wait<DS_STAGES - 2>();
       const unsigned char* st = ring + (size_t)((k - k0) % DS_STAGES) * stage_bytes;
-      fwd_read_row<REV, NC, SRC>(J, st, cpitch, xo);
-      fwd_read_row<REV, NC, SRC>(J, st + row_bytes, cpitch, xn);
+      fwd_read_row<REV, NC, SRC, ILV>(J, st, cpitch, xo);
+      fwd_read_row<REV, NC, SRC, ILV>(J, st + row_bytes, cpitch, xn);
       #pragma unroll
       for (int c = 0; c < NC; ++c)
         #pragma unroll
@@ -543,8 +645,8 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const voi
         if (TMA && tma) issue_tma(issued, (uint32_t)((issued - k0) % DS_STAGES));
         else {
           unsigned char* sn = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
-          fwd_issue_row<NC, SRC>(J, g, image, coef, 2 * issued - 1, sn, cpitch);
-          fwd_issue_row<NC, SRC>(J, g, image, coef, 2 * issued, sn + row_bytes, cpitch);
+          fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, sn, cpitch);
+          fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, sn + row_bytes, cpitch);
         }
       }
       cp_commit(); ++issued;
@@ -621,8 +723,8 @@ __device__ __forceinline__ void inv_read_pair(const unsigned char* st, typename 
 // differ only on exact halves, which zero-decomposition 9/7 components produce systematically.
 __device__ __forceinline__ int round_haz(float t) { return __float2int_rn(t); }
 
-template <bool REV, int NC, int SRC>
-__device__ __forceinline__ void inv_store_row(const DwtJob& J, const StripGeom& g, void* image, uint32_t* coef,
+template <bool REV, int NC, int SRC, bool ILV>
+__device__ __forceinline__ void inv_store_row(const DwtJob& J, const StripGeom& g, const ImgView* V, uint32_t* coef,
                                               int v, typename Tp<REV>::T (&x)[NC][4])
 {
   constexpr bool FIRST = SRC != SRC_COEF;     // the full-resolution side is the image
@@ -702,51 +804,65 @@ __device__ __forceinline__ void inv_store_row(const DwtJob& J, const StripGeom& 
   // 8 / 16-bit containers: clamp to the component's range as the reference's file writers do
   // (gen_cvrt_32b*_to_*, yuv_out::write: src/apps/others/ojph_img_io.cpp:99-235, :1477-1516)
   const int smax = (1 << J.bit_depth) - 1;
+  if constexpr (ILV) {                        // four whole pixels at a pixel-aligned address: vectors (ilv_store)
+    constexpr uint32_t ES = (SRC == SRC_U16) ? 2u : (SRC == SRC_U8 ? 1u : 4u);
+    unsigned char* p = V[0].org + (uint32_t)(v - g.y0) * (uint32_t)V[0].pitch + (uint32_t)cx * V[0].step;
+    if (all4 && ((uint32_t)(size_t)p & (4u * ES - 1u)) == 0) {
+      uint32_t q[3][4];
+      #pragma unroll
+      for (int k = 0; k < 3; ++k)
+        #pragma unroll
+        for (int i = 0; i < 4; ++i) q[k][i] = SRC == SRC_I32 ? (uint32_t)out[k][i] : (uint32_t)min(max(out[k][i], 0), smax);
+      if (V[0].step == 3u * ES) ilv_store<3, ES>(p, q); else ilv_store<4, ES>(p, q);
+      return;
+    }
+  }
   #pragma unroll
   for (int k = 0; k < NC; ++k) {
-    // 32-bit byte offset into the (256-byte aligned) image buffer
-    const uint32_t eidx = (uint32_t)(v - g.y0) * J.full_stride[k] + (uint32_t)cx;
-    unsigned char* base = reinterpret_cast<unsigned char*>(image);
+    // the row, then 32-bit byte offsets along it; a lane's first column lies left of the resolution (cx < 0) only
+    // when has[0] is false, so the vector stores below never see the wrapped offset
+    unsigned char* row = V[k].org + (uint32_t)(v - g.y0) * (uint32_t)V[k].pitch;
+    const uint32_t step = V[k].step;
+    unsigned char* p = row + (uint32_t)cx * step;
+    const uint32_t a = (uint32_t)(size_t)p;
     if (SRC == SRC_U16) {
-      const uint32_t o = (uint32_t)J.full_off[k] + 2u * eidx;
-
       uint32_t q[4];
       #pragma unroll
       for (int i = 0; i < 4; ++i) q[i] = (uint32_t)min(max(out[k][i], 0), smax);
-      if (all4 && (o & 7u) == 0) *reinterpret_cast<uint2*>(base + o) = make_uint2(q[0] | (q[1] << 16), q[2] | (q[3] << 16));
+      if (all4 && step == 2u && (a & 7u) == 0) *reinterpret_cast<uint2*>(p) = make_uint2(q[0] | (q[1] << 16), q[2] | (q[3] << 16));
       else {
         #pragma unroll
-        for (int i = 0; i < 4; ++i) if (g.has[i]) *reinterpret_cast<unsigned short*>(base + (o + 2u * (uint32_t)i)) = (unsigned short)q[i];
+        for (int i = 0; i < 4; ++i) if (g.has[i]) *reinterpret_cast<unsigned short*>(row + (uint32_t)(cx + i) * step) = (unsigned short)q[i];
       }
     } else if (SRC == SRC_U8) {
-      const uint32_t o = (uint32_t)J.full_off[k] + eidx;
       uint32_t q[4];
       #pragma unroll
       for (int i = 0; i < 4; ++i) q[i] = (uint32_t)min(max(out[k][i], 0), smax);
-      if (all4 && (o & 3u) == 0) *reinterpret_cast<uint32_t*>(base + o) = q[0] | (q[1] << 8) | (q[2] << 16) | (q[3] << 24);
+      if (all4 && step == 1u && (a & 3u) == 0) *reinterpret_cast<uint32_t*>(p) = q[0] | (q[1] << 8) | (q[2] << 16) | (q[3] << 24);
       else {
         #pragma unroll
-        for (int i = 0; i < 4; ++i) if (g.has[i]) base[o + (uint32_t)i] = (unsigned char)q[i];
+        for (int i = 0; i < 4; ++i) if (g.has[i]) row[(uint32_t)(cx + i) * step] = (unsigned char)q[i];
       }
     } else {
-      const uint32_t o = (uint32_t)J.full_off[k] + 4u * eidx;
-      if (all4 && (o & 15u) == 0)
-        *reinterpret_cast<uint4*>(base + o) = make_uint4((uint32_t)out[k][0], (uint32_t)out[k][1], (uint32_t)out[k][2], (uint32_t)out[k][3]);
+      if (all4 && step == 4u && (a & 15u) == 0)
+        *reinterpret_cast<uint4*>(p) = make_uint4((uint32_t)out[k][0], (uint32_t)out[k][1], (uint32_t)out[k][2], (uint32_t)out[k][3]);
       else {
         #pragma unroll
-        for (int i = 0; i < 4; ++i) if (g.has[i]) *reinterpret_cast<int*>(base + (o + 4u * (uint32_t)i)) = out[k][i];
+        for (int i = 0; i < 4; ++i) if (g.has[i]) *reinterpret_cast<int*>(row + (uint32_t)(cx + i) * step) = out[k][i];
       }
     }
   }
 }
 
-template <bool REV, int NC, int SRC>
+template <bool REV, int NC, int SRC, bool ILV>
 __global__ void __launch_bounds__(DS_WARPS * 32, (REV || NC == 1) ? 5 : 3)
-dwt_inv_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, void* __restrict__ image,
+dwt_inv_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const ImgComp* __restrict__ img,
                       uint32_t* __restrict__ coef)
 {
   typedef typename Tp<REV>::T T;
+  constexpr bool FIRSTK = SRC != SRC_COEF;
   __shared__ DwtJob sj;
+  __shared__ ImgView sv[FIRSTK ? NC : 1];
   {
     uint32_t ji = find_job(jobs, njobs, blockIdx.x);
     const uint32_t* s = reinterpret_cast<const uint32_t*>(&jobs[ji]);
@@ -754,7 +870,12 @@ dwt_inv_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, void* __r
     for (uint32_t i = threadIdx.x; i < sizeof(DwtJob) / 4; i += blockDim.x) d[i] = s[i];
   }
   __syncthreads();
+  if (FIRSTK) {
+    if (threadIdx.x < NC) sv[threadIdx.x] = img_view(img, sj, threadIdx.x);
+    __syncthreads();
+  }
   const DwtJob& J = sj;
+  const ImgView* V = sv;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const uint32_t cta = blockIdx.x - J.cta_base;
   const uint32_t strips_per_row = (J.tiles_x + DS_WARPS - 1) / DS_WARPS;
@@ -808,8 +929,8 @@ dwt_inv_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, void* __r
         }
       if (issued <= j1) inv_issue_pair<NC>(J, g, coef, issued, ring + (size_t)((issued - j0) % NS) * stage_bytes);
       cp_commit(); ++issued;
-      inv_store_row<REV, NC, SRC>(J, g, image, coef, 2 * j - 1, xo);
-      inv_store_row<REV, NC, SRC>(J, g, image, coef, 2 * j, xn);
+      inv_store_row<REV, NC, SRC, ILV>(J, g, V, coef, 2 * j - 1, xo);
+      inv_store_row<REV, NC, SRC, ILV>(J, g, V, coef, 2 * j, xn);
     }
   } else {
     T s1[NC][4], d1[NC][4], xe[NC][4];      // s1[j-1], d1[j-2], x_e[j-2]
@@ -835,8 +956,8 @@ dwt_inv_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, void* __r
         }
       if (issued <= j1) inv_issue_pair<NC>(J, g, coef, issued, ring + (size_t)((issued - j0) % NS) * stage_bytes);
       cp_commit(); ++issued;
-      inv_store_row<REV, NC, SRC>(J, g, image, coef, 2 * j - 3, xo);
-      inv_store_row<REV, NC, SRC>(J, g, image, coef, 2 * j - 2, xn);
+      inv_store_row<REV, NC, SRC, ILV>(J, g, V, coef, 2 * j - 3, xo);
+      inv_store_row<REV, NC, SRC, ILV>(J, g, V, coef, 2 * j - 2, xn);
     }
   }
 }
@@ -846,26 +967,47 @@ bool dwt_use_tma() {
   return v;
 }
 template <bool REV, int NC, int SRC>
-void launch_fwd(const DwtJob* jobs, uint32_t njobs, uint32_t ctas, const void* image, uint32_t* coef, cudaStream_t st) {
+void launch_fwd(const DwtJob* jobs, uint32_t njobs, uint32_t ctas, const ImgComp* img, uint32_t* coef, cudaStream_t st,
+                uint32_t layout) {
   const size_t slot = (SRC == SRC_U8 || SRC == SRC_U16) ? 8 : 16;
-  if (dwt_use_tma() && (SRC == SRC_U16 || SRC == SRC_COEF)) {          // bulk-copy staging
-    auto k = dwt_fwd_stream_kernel<REV, NC, SRC, (SRC == SRC_U16 || SRC == SRC_COEF)>;
+  if constexpr (NC == 3 && SRC != SRC_COEF) {
+    if (layout == IMG_CALLER_ILV) {
+      auto k = dwt_fwd_stream_kernel<REV, NC, SRC, false, true>;
+      const size_t smem = (size_t)DS_WARPS * DS_STAGES * 2 * 32 * (4 * slot);     // 16 ES bytes per lane and row
+      cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
+      return;
+    }
+  }
+  // bulk-copy staging reads up to 16 bytes past a row's last sample: the codec's own buffer has the slack, a caller's
+  // may not
+  if (dwt_use_tma() && (SRC == SRC_U16 || SRC == SRC_COEF) && (SRC == SRC_COEF || layout == IMG_OWN)) {
+    auto k = dwt_fwd_stream_kernel<REV, NC, SRC, (SRC == SRC_U16 || SRC == SRC_COEF), false>;
     const size_t smem = (size_t)DS_WARPS * DS_STAGES * 2 * NC * (32 * slot + 16);
     cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, image, coef);
+    OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
     return;
   }
-  auto k = dwt_fwd_stream_kernel<REV, NC, SRC, false>;
+  auto k = dwt_fwd_stream_kernel<REV, NC, SRC, false, false>;
   const size_t smem = (size_t)DS_WARPS * DS_STAGES * 2 * NC * 32 * slot;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, image, coef);
+  OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
 }
 template <bool REV, int NC, int SRC>
-void launch_inv(const DwtJob* jobs, uint32_t njobs, uint32_t ctas, void* image, uint32_t* coef, cudaStream_t st) {
-  auto k = dwt_inv_stream_kernel<REV, NC, SRC>;
+void launch_inv(const DwtJob* jobs, uint32_t njobs, uint32_t ctas, const ImgComp* img, uint32_t* coef, cudaStream_t st,
+                uint32_t layout) {
   const size_t smem = (size_t)DS_WARPS * ((NC == 3) ? DS_STAGES - 1 : DS_STAGES) * NC * 4 * 32 * 8;
+  if constexpr (NC == 3 && SRC != SRC_COEF) {
+    if (layout == IMG_CALLER_ILV) {
+      auto k = dwt_inv_stream_kernel<REV, NC, SRC, true>;
+      cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
+      return;
+    }
+  }
+  auto k = dwt_inv_stream_kernel<REV, NC, SRC, false>;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, image, coef);
+  OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
 }
 
 } // namespace
@@ -893,10 +1035,10 @@ void dwt_stream_tiling(uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, bool re
 }
 
 void launch_dwt_fwd_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                           uint32_t ncomp, bool first, uint32_t src_type, const void* image, uint32_t* coef, cudaStream_t st)
+                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, uint32_t img_layout, uint32_t* coef, cudaStream_t st)
 {
   if (total_ctas == 0) return;
-#define OJB_FWD(REV, NC, SRC) launch_fwd<REV, NC, SRC>(jobs, njobs, total_ctas, image, coef, st)
+#define OJB_FWD(REV, NC, SRC) launch_fwd<REV, NC, SRC>(jobs, njobs, total_ctas, img, coef, st, img_layout)
 #define OJB_FWD_SRC(REV, NC) do { if (src_type == SRC_U8) OJB_FWD(REV, NC, SRC_U8); else if (src_type == SRC_U16) OJB_FWD(REV, NC, SRC_U16); \
                                   else OJB_FWD(REV, NC, SRC_I32); } while (0)
   if (reversible) {
@@ -911,10 +1053,10 @@ void launch_dwt_fwd_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ct
 }
 
 void launch_dwt_inv_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                           uint32_t ncomp, bool first, uint32_t src_type, void* image, uint32_t* coef, cudaStream_t st)
+                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, uint32_t img_layout, uint32_t* coef, cudaStream_t st)
 {
   if (total_ctas == 0) return;
-#define OJB_INV(REV, NC, SRC) launch_inv<REV, NC, SRC>(jobs, njobs, total_ctas, image, coef, st)
+#define OJB_INV(REV, NC, SRC) launch_inv<REV, NC, SRC>(jobs, njobs, total_ctas, img, coef, st, img_layout)
 #define OJB_INV_SRC(REV, NC) do { if (src_type == SRC_U8) OJB_INV(REV, NC, SRC_U8); else if (src_type == SRC_U16) OJB_INV(REV, NC, SRC_U16); \
                                   else OJB_INV(REV, NC, SRC_I32); } while (0)
   if (reversible) {

@@ -304,7 +304,7 @@ int ojb_dec_decode_raster(ojb_decoder* d, uint32_t layout, void* payload, uint64
       for (uint32_t c = 0; c < nc; ++c) { planes[c] = p; p += (size_t)D.img_w[c] * D.img_h[c] * es; }
       D.decode(planes.data(), nullptr, false);
     } else {
-      D.decode(nullptr, nullptr, true);
+      D.decode(nullptr, nullptr, false);
       d->d_raster.reserve(std::max<uint64_t>(need, 16));
       launch_raster_pack(d->d_raster.p, D.d_image.p, pl, nc, es, D.img_w[0], D.img_h[0], D.stream);
       cuda_check(cudaMemcpyAsync(payload, d->d_raster.p, need, cudaMemcpyDeviceToHost, D.stream), "download");
@@ -334,6 +334,28 @@ static void upload_frame(Encoder& E, const void* const* planes, const uint32_t* 
   }
   cuda_check(cudaStreamSynchronize(E.stream), "upload sync");
 }
+// the caller's image (ojb_device_image) checked against the component sizes of ojb_frame_info
+static void caller_image(const CodecBase& cb, const ojb_device_image* in, std::vector<ImgComp>& comps) {
+  const uint32_t nc = cb.params.num_comps();
+  const uint64_t es = cb.img_type == ST_U8 ? 1u : (cb.img_type == ST_U16 ? 2u : 4u);
+  comps.assign(nc, ImgComp());
+  for (uint32_t c = 0; c < nc; ++c) {
+    const uint64_t base = in ? (uint64_t)(uintptr_t)in->base[c] : 0, pitch = in ? in->row_pitch[c] : 0;
+    if (base == 0) fail(0x000B003B, "component %u: null base address", c);
+    if (base % es || pitch % es)
+      fail(0x000B003B, "component %u: base address or row pitch is not a multiple of the %u-byte sample", c, (uint32_t)es);
+    const uint32_t col = in->col_stride[c], w = cb.img_w[c], h = cb.img_h[c];
+    if (col == 0) fail(0x000B003C, "component %u: column stride 0", c);
+    comps[c].base = base; comps[c].pitch = pitch; comps[c].col = col; comps[c].pad = 0;
+    if (w == 0 || h == 0) continue;
+    const unsigned __int128 row = ((unsigned __int128)(w - 1) * col + 1) * es;
+    if (h > 1 && (unsigned __int128)pitch < row)
+      fail(0x000B003D, "component %u: row pitch of %llu bytes is smaller than one row of %u samples at column stride %u",
+           c, (unsigned long long)pitch, w, col);
+    if ((unsigned __int128)(h - 1) * pitch + row >= ((unsigned __int128)1 << 32))
+      fail(0x000B003E, "component %u: the %u x %u samples span 4 GiB or more (offsets from base are formed in 32 bits)", c, w, h);
+  }
+}
 static void read_band(CodecBase& cb, uint32_t tile, uint32_t comp, uint32_t res, uint32_t band, uint32_t* out,
                       uint32_t* bw, uint32_t* bh) {
   if (tile >= cb.layout.tiles.size() || comp >= cb.params.num_comps() || res > cb.params.decomps(comp) || band > 3)
@@ -361,10 +383,20 @@ int ojb_enc_upload_frame(ojb_encoder* e, const void* const* planes, const uint32
     upload_frame(e->enc, planes, strides);
   });
 }
+int ojb_enc_encode_device(ojb_encoder* e, const ojb_device_image* in, void* cuda_stream,
+                          uint8_t* out, uint64_t out_cap, uint64_t* out_len, int out_on_device) {
+  return guarded_on(e->device, [&] {
+    if (!e->configured) fail(0x000B003F, "encoder is not configured");
+    std::vector<ImgComp> comps;
+    caller_image(e->enc, in, comps);
+    e->enc.use_caller_image(comps.data(), static_cast<cudaStream_t>(cuda_stream));
+    *out_len = e->enc.encode(nullptr, nullptr, true, out, (size_t)out_cap, out_on_device != 0);
+  });
+}
 int ojb_enc_encode_resident(ojb_encoder* e, uint8_t* out, uint64_t out_cap, uint64_t* out_len, int out_on_device) {
   return guarded_on(e->device, [&] {
     if (!e->configured) fail(0x000B0013, "encoder is not configured");
-    *out_len = e->enc.encode(nullptr, nullptr, true, out, (size_t)out_cap, out_on_device != 0);
+    *out_len = e->enc.encode(nullptr, nullptr, false, out, (size_t)out_cap, out_on_device != 0);
   });
 }
 uint32_t ojb_enc_kernel_launches(ojb_encoder* e) { return e->enc.last_launches; }
@@ -561,6 +593,15 @@ const int32_t* ojb_dec_pull(ojb_decoder* d, uint32_t* comp_num) {
 int ojb_dec_decode_resident(ojb_decoder* d) {
   return guarded_on(d->device, [&] {
     if (!d->have_headers) fail(0x000B0015, "read_headers has not been called");
+    d->dec.decode(nullptr, nullptr, false);
+  });
+}
+int ojb_dec_decode_device(ojb_decoder* d, const ojb_device_image* out, void* cuda_stream) {
+  return guarded_on(d->device, [&] {
+    if (!d->have_headers) fail(0x000B003F, "read_headers has not been called");
+    std::vector<ImgComp> comps;
+    caller_image(d->dec, out, comps);
+    d->dec.use_caller_image(comps.data(), static_cast<cudaStream_t>(cuda_stream));
     d->dec.decode(nullptr, nullptr, true);
   });
 }

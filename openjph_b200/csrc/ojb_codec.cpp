@@ -41,6 +41,7 @@ CodecBase::CodecBase() {
   CK(cudaStreamCreateWithFlags(&side.st, cudaStreamNonBlocking));
   CK(cudaEventCreateWithFlags(&side.fork, cudaEventDisableTiming));
   CK(cudaEventCreateWithFlags(&side.join, cudaEventDisableTiming));
+  CK(cudaEventCreateWithFlags(&ev_caller, cudaEventDisableTiming));
   unsigned hc = std::thread::hardware_concurrency();
   host_threads = hc == 0 ? 4u : std::min(8u, hc);
   for (int i = 0; i < EV_MAX; ++i) CK(cudaEventCreate(&ev[i]));
@@ -56,6 +57,7 @@ CodecBase::~CodecBase() {
   for (int i = 0; i < EV_MAX; ++i) if (ev[i]) cudaEventDestroy(ev[i]);
   if (side.fork) cudaEventDestroy(side.fork);
   if (side.join) cudaEventDestroy(side.join);
+  if (ev_caller) cudaEventDestroy(ev_caller);
   if (side.st) cudaStreamDestroy(side.st);
   if (stream) cudaStreamDestroy(stream);
 }
@@ -100,6 +102,33 @@ void CodecBase::plan_image(uint32_t sample_type) {
   }
   img_bytes = off + 256;
   d_image.reserve(img_bytes);
+  if (nc > IMG_SLOTS) fail(0x000B0008, "%u components: the frame interface carries at most %u", nc, (uint32_t)IMG_SLOTS);
+  std::vector<ImgComp> own(IMG_SLOTS);
+  for (uint32_t c = 0; c < nc; ++c) {
+    own[c].base = (uint64_t)(size_t)(d_image.as<uint8_t>() + img_off[c]);
+    own[c].pitch = (uint64_t)img_w[c] * esize_of(sample_type); own[c].col = 1; own[c].pad = 0;
+  }
+  d_img.reserve(2 * IMG_SLOTS * sizeof(ImgComp));
+  h_img.reserve(IMG_SLOTS * sizeof(ImgComp));
+  CK(cudaMemcpy(d_img.p, own.data(), IMG_SLOTS * sizeof(ImgComp), cudaMemcpyHostToDevice));
+}
+
+void CodecBase::use_caller_image(const ImgComp* comps, cudaStream_t caller_stream) {
+  const uint32_t nc = params.num_comps(), es = esize_of(img_type);
+  memcpy(h_img.p, comps, (size_t)nc * sizeof(ImgComp));
+  caller_layout = IMG_CALLER;
+  if (nc >= 3 && (comps[0].col == 3 || comps[0].col == 4)) {
+    bool adj = true;
+    for (uint32_t k = 1; k < 3; ++k)
+      adj = adj && comps[k].base == comps[0].base + k * es && comps[k].pitch == comps[0].pitch && comps[k].col == comps[0].col;
+    if (adj) caller_layout = IMG_CALLER_ILV;
+  }
+  CK(cudaEventRecord(ev_caller, caller_stream));
+  CK(cudaStreamWaitEvent(stream, ev_caller, 0));
+}
+void CodecBase::enqueue_caller_image() {
+  launch_ctrl_copy(const_cast<ImgComp*>(img_slot(true)), h_img.p, (size_t)params.num_comps() * sizeof(ImgComp), stream);
+  ++last_launches;
 }
 
 // the register-streaming kernels take a level when it splits both ways with the built-in 5/3 or 9/7, the resolution is
@@ -275,7 +304,6 @@ void CodecBase::build_dwt_jobs(bool forward) {
       if (P.decomps(c) != P.decomps(0) || P.wavelet_of(c) != P.wavelet_of(0) || P.dfs_of(c) != P.dfs_of(0))
         fail(0x000B0006, "the colour transform needs one coding style for the first three components");
   jobs.assign(nlev, std::vector<JobGroup>());
-  uint32_t es = esize_of(img_type);
   for (uint32_t li = 0; li < nlev; ++li) {
     // groups per wavelet w (0: 5/3, 1: 9/7): [4w+0] streaming 3-comp first, [4w+1] streaming 1-comp first,
     // [4w+2] streaming inner levels, [4w+3] general
@@ -329,8 +357,7 @@ void CodecBase::build_dwt_jobs(bool forward) {
             // the resolution's rectangle sits at (ceil(x0 / 2^s) - ceil(XO / (dx 2^s))) in the output plane
             uint32_t fx, fy; P.res_downsamp(c + i, top, fx, fy);
             uint32_t cx0 = div_ceil(P.XOsiz, P.comps[c + i].dx * fx), cy0 = div_ceil(P.YOsiz, P.comps[c + i].dy * fy);
-            j.full_off[i] = img_off[c + i] + ((uint64_t)(rr.rect.y0 - cy0) * img_w[c + i] + (rr.rect.x0 - cx0)) * es;
-            j.full_stride[i] = img_w[c + i];
+            j.img_comp[i] = c + i; j.img_x[i] = rr.rect.x0 - cx0; j.img_y[i] = rr.rect.y0 - cy0;
           } else { j.full_off[i] = rr.plane_off; j.full_stride[i] = rr.plane_stride; }
           if (r > 0) {
             const ResGeom& lo = tc.res[r - 1];
@@ -676,7 +703,7 @@ int32_t* Encoder::exchange(const int32_t* line_written, uint32_t& next_comp) {
   return line_buf.data();
 }
 
-size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool planes_on_device,
+size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool caller_image,
                        uint8_t* out, size_t out_cap, bool out_on_device)
 {
   const Params& P = params;
@@ -688,13 +715,12 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     for (uint32_t c = 0; c < nc; ++c) {
       uint8_t* d = d_image.as<uint8_t>() + img_off[c];
       uint32_t st = strides ? strides[c] : img_w[c];
-      cudaMemcpyKind kind = planes_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
       if (st == img_w[c])
-        CK(cudaMemcpyAsync(d, planes[c], (size_t)img_w[c] * img_h[c] * es, kind, stream));
+        CK(cudaMemcpyAsync(d, planes[c], (size_t)img_w[c] * img_h[c] * es, cudaMemcpyHostToDevice, stream));
       else
         for (uint32_t y = 0; y < img_h[c]; ++y)
           CK(cudaMemcpyAsync(d + (size_t)y * img_w[c] * es, (const uint8_t*)planes[c] + (size_t)y * st * es,
-                             (size_t)img_w[c] * es, kind, stream));
+                             (size_t)img_w[c] * es, cudaMemcpyHostToDevice, stream));
     }
   }
   mark(1);
@@ -772,15 +798,17 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   // rank's blocks then travel to the writer --, PHASE_BACK on the writer starts behind it)
   auto enqueue_front = [&] {
   CK(cudaMemsetAsync(d_status.p, 0, 16, stream));
+  if (caller_image) enqueue_caller_image();
   if (phase != PHASE_BACK)
   for (size_t li = 0; li < jobs.size(); ++li)
     for (const JobGroup& g : jobs[li]) {
       if (g.stream)
         launch_dwt_fwd_stream(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                              g.first, img_type, d_image.p, d_coef.as<uint32_t>(), stream);
+                              g.first, img_type, img_slot(caller_image), caller_image ? caller_layout : (uint32_t)IMG_OWN,
+                              d_coef.as<uint32_t>(), stream);
       else
         launch_dwt_fwd(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                       d_image.p, d_coef.as<uint32_t>(), stream, wide);
+                       img_slot(caller_image), d_coef.as<uint32_t>(), stream, wide);
       ++last_launches;
     }
   mark(2);
@@ -833,10 +861,12 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
       mark(6);
       };
       // resident form (frame already in HBM, codestream stays there): nothing in the call depends on host data, so
-      // the whole thing replays as a graph
+      // the whole thing replays as a graph (a caller's image is named by the control block the graph copies in,
+      // so its addresses are not part of the key)
       if (attempt == 0 && planes == nullptr && out_on_device && phase == PHASE_ALL)
         run_frame({ (uint64_t)(size_t)dev_out, cap, (uint64_t)nb, (uint64_t)num_fast_blocks, (uint64_t)(size_t)d_slots.p, (uint64_t)(size_t)d_coef.p,
-                    rc_frame ? target_bytes : 0, (uint64_t)(size_t)d_rc.p, (uint64_t)(size_t)d_work.p }, enqueue_all);
+                    rc_frame ? target_bytes : 0, (uint64_t)(size_t)d_rc.p, (uint64_t)(size_t)d_work.p,
+                    (uint64_t)(size_t)img_slot(caller_image), (uint64_t)(caller_image ? caller_layout : (uint32_t)IMG_OWN) }, enqueue_all);
       else enqueue_all();
       CK(cudaStreamSynchronize(stream));
       CK(cudaGetLastError());
@@ -1295,7 +1325,7 @@ void Decoder::parse_tiles() {
   }
 }
 
-uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool planes_on_device) {
+uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool caller_image) {
   const Params& P = params;
   uint32_t nc = P.num_comps(), es = esize_of(img_type), D = P.num_decomps;
   last_launches = 0;
@@ -1377,15 +1407,17 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool plan
   last_launches += 1 + (nfast ? 1 : 0) + (nfast < nb ? 1 : 0);
   mark(3);
   if (nb) { launch_ctrl_copy(h_bstatus.p, d_bstatus.p, (size_t)nb * 4, stream); ++last_launches; }
+  if (caller_image) enqueue_caller_image();
   // synthesis, coarsest level first
   for (size_t li = jobs.size(); li-- > 0; )
     for (const JobGroup& g : jobs[li]) {
       if (g.stream)
         launch_dwt_inv_stream(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                              g.first, img_type, d_image.p, d_coef.as<uint32_t>(), stream);
+                              g.first, img_type, img_slot(caller_image), caller_image ? caller_layout : (uint32_t)IMG_OWN,
+                              d_coef.as<uint32_t>(), stream);
       else
         launch_dwt_inv(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                       d_image.p, d_coef.as<uint32_t>(), stream, wide);
+                       img_slot(caller_image), d_coef.as<uint32_t>(), stream, wide);
       ++last_launches;
     }
   (void)D;
@@ -1394,22 +1426,23 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool plan
     for (uint32_t c = 0; c < nc; ++c) {
       const uint8_t* s = d_image.as<uint8_t>() + img_off[c];
       uint32_t st = strides ? strides[c] : img_w[c];
-      cudaMemcpyKind kind = planes_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
       if (st == img_w[c])
-        CK(cudaMemcpyAsync(planes[c], s, (size_t)img_w[c] * img_h[c] * es, kind, stream));
+        CK(cudaMemcpyAsync(planes[c], s, (size_t)img_w[c] * img_h[c] * es, cudaMemcpyDeviceToHost, stream));
       else
         for (uint32_t y = 0; y < img_h[c]; ++y)
           CK(cudaMemcpyAsync((uint8_t*)planes[c] + (size_t)y * st * es, s + (size_t)y * img_w[c] * es,
-                             (size_t)img_w[c] * es, kind, stream));
+                             (size_t)img_w[c] * es, cudaMemcpyDeviceToHost, stream));
     }
   }
   mark(5);
   };
-  // resident form (codestream in HBM, image stays there): what follows the host parse replays as a graph -- the
-  // frame's own data (block records, lengths, offsets) reaches the kernels through the pinned record buffer
+  // resident form (codestream in HBM, image stays there or goes to the caller's memory): what follows the host parse
+  // replays as a graph -- the frame's own data (block records, lengths, offsets, where the caller's image is) reaches
+  // the kernels through pinned buffers the graph copies in
   if (planes == nullptr && dev_cs != nullptr)
     run_frame({ (uint64_t)(size_t)cs_dev, (uint64_t)nb, (uint64_t)(nfast != 0), (uint64_t)(nfast < nb), (uint64_t)cleanup_only, (uint64_t)dec_out,
-                (uint64_t)(size_t)d_scratch.p, (uint64_t)skip_recon, (uint64_t)(size_t)hy, (uint64_t)(size_t)d_coef.p, (uint64_t)(size_t)d_image.p }, enqueue);
+                (uint64_t)(size_t)d_scratch.p, (uint64_t)skip_recon, (uint64_t)(size_t)hy, (uint64_t)(size_t)d_coef.p, (uint64_t)(size_t)d_image.p,
+                (uint64_t)(size_t)img_slot(caller_image), (uint64_t)(caller_image ? caller_layout : (uint32_t)IMG_OWN) }, enqueue);
   else enqueue();
   CK(cudaStreamSynchronize(stream));
   CK(cudaGetLastError());

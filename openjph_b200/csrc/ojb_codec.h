@@ -74,6 +74,19 @@ public:
   uint32_t skip_read = 0, skip_recon = 0;
   size_t img_bytes = 0;
   void plan_image(uint32_t sample_type);
+  // The image as the first-level DWT jobs reach it: one ImgComp per component in device memory.  Slot 0 describes
+  // d_image (written by plan_image), slot 1 the caller's memory of a *_device call: the frame's own work copies it
+  // from h_img, so a captured frame graph replays with whatever buffers the next call names.
+  enum { IMG_SLOTS = 16 };
+  DeviceBuf d_img;
+  PinnedBuf h_img;
+  cudaEvent_t ev_caller = nullptr;
+  uint32_t caller_layout = IMG_CALLER;   // of the image in slot 1 (IMG_CALLER_ILV: see launch_dwt_fwd_stream)
+  const ImgComp* img_slot(bool caller) const { return reinterpret_cast<const ImgComp*>(d_img.p) + (caller ? IMG_SLOTS : 0); }
+  // the next frame call reads (encoder) or writes (decoder) the caller's memory described by comps[num_comps], after
+  // the work enqueued so far on caller_stream (0: the legacy default stream)
+  void use_caller_image(const ImgComp* comps, cudaStream_t caller_stream);
+  void enqueue_caller_image();         // inside the frame's work: h_img -> slot 1
   DeviceBuf d_coef;                    // coefficient arena (32-bit words; 64-bit elements in wide mode)
   bool wide = false;                   // some component needs more than 32 bits: every plane holds 64-bit elements, general kernels only
   // DWT jobs per level (index 0: full resolution level D, ...), uploaded once
@@ -114,9 +127,10 @@ class Encoder : public CodecBase {
 public:
   // finalises parameters, builds geometry and device arenas, produces the main header
   void configure(const Params& p, uint32_t sample_type);
-  // encode one frame whose component planes are on the host (pinned or pageable) or on the
-  // device; planes[c] points at sample (0,0) of component c, stride in samples
-  size_t encode(const void* const* planes, const uint32_t* strides, bool planes_on_device,
+  // encode one frame whose component planes are on the host (pinned or pageable; planes[c] points at sample (0,0) of
+  // component c, stride in samples), already in d_image (planes == nullptr), or in the caller's device memory
+  // (caller_image: described by use_caller_image)
+  size_t encode(const void* const* planes, const uint32_t* strides, bool caller_image,
                 uint8_t* out, size_t out_cap, bool out_on_device);
   uint32_t status_flags = 0;
   // row regions (ojb_shard.cpp): the frame call split at the point where code-block bytes change hands
@@ -202,8 +216,9 @@ public:
   std::vector<uint8_t> block_res;       // per block: how many resolutions lie above its own (D_c - r)
   std::vector<uint8_t> block_wanted;    // with a tile mask: the block belongs to one of this object's tiles
   void info(FrameInfo& fi) const;
-  // decode into planes (host or device); returns number of code-blocks that failed to decode
-  uint32_t decode(void* const* planes, const uint32_t* strides, bool planes_on_device);
+  // decode into host planes, into d_image (planes == nullptr) or into the caller's device memory (caller_image:
+  // described by use_caller_image); returns number of code-blocks that failed to decode
+  uint32_t decode(void* const* planes, const uint32_t* strides, bool caller_image);
   uint32_t failed_blocks = 0;
   const uint8_t* j2c = nullptr; size_t j2c_len = 0; size_t first_sot = 0;
   const uint8_t* dev_cs = nullptr;     // optional: the same bytes already resident in HBM (+32 bytes slack)

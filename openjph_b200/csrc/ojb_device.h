@@ -129,6 +129,18 @@ enum : uint32_t {       // DecBlock output modes
 // ---- DWT --------------------------------------------------------------------------------
 enum : uint32_t { SRC_U8 = 0, SRC_U16 = 1, SRC_I32 = 2, SRC_COEF = 3 };
 
+// Where the samples of one image component are: sample (x, y) sits at base + y * pitch + x * col * (sample size).
+// The first-level jobs of the DWT kernels reach the image only through an array of these, one per component (a
+// per-frame control block in device memory): the codec's own image buffer (tight rows, col = 1) or the caller's
+// memory (any pitch, planar or interleaved).  The streaming kernels form offsets from base in 32 bits: every
+// component they address spans fewer than 2^32 bytes.
+struct ImgComp {
+  uint64_t base;        // device address of sample (0, 0)
+  uint64_t pitch;       // bytes from one row to the next
+  uint32_t col;         // samples from one column to the next
+  uint32_t pad;
+};
+
 // one analysis (or synthesis) level of one tile-component (or of 3 colour components at once
 // for the first level when the colour transform is used)
 #define DWT_MAX_STEPS 8        // = the halo of the general kernels' tile (DW_H): one sample per lifting step
@@ -137,8 +149,10 @@ struct DwtJob {
   uint32_t w, h;          // size
   uint32_t x0, y0;        // origin (only parity and band-origin arithmetic matter)
   // source / destination of the full-resolution samples
-  uint64_t full_off[3];   // word offset in arena (SRC_COEF) or byte offset in image buffer
-  uint32_t full_stride[3];// in samples
+  uint64_t full_off[3];   // not first: word offset in the arena
+  uint32_t full_stride[3];// not first: in samples
+  // first: component img_comp[i] of the image (ImgComp), the resolution's origin at column img_x[i], row img_y[i]
+  uint32_t img_comp[3], img_x[3], img_y[3];
   // LL output (next level input) -- arena word offsets
   uint64_t ll_off[3];
   uint32_t ll_stride[3];

@@ -36,20 +36,24 @@ void launch_dec_merge(DecBlock* blocks, const DecBlock* proto, const DecDyn* dyn
 void launch_ht_decode_wide(const DecBlock* blocks, uint32_t nblocks, uint32_t max_width, const uint8_t* codestream,
                            uint32_t* coef, const uint16_t* tables, bool signmag, uint32_t* block_status, cudaStream_t st);
 
-// forward / inverse DWT levels (dwt_fwd.cu / dwt_inv.cu).  jobs live in device memory.
+// forward / inverse DWT levels (dwt_fwd.cu / dwt_inv.cu).  jobs live in device memory; the first level reaches the
+// image through img (device memory, one ImgComp per component)
 // wide: 64-bit samples and sign-magnitude words (reversible, precision > 32 bits); offsets and strides count elements
 void launch_dwt_fwd(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                    uint32_t max_ncomp, const void* image, uint32_t* coef, cudaStream_t st, bool wide = false);
+                    uint32_t max_ncomp, const ImgComp* img, uint32_t* coef, cudaStream_t st, bool wide = false);
 void launch_dwt_inv(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                    uint32_t max_ncomp, void* image, uint32_t* coef, cudaStream_t st, bool wide = false);
-// register-streaming fast path (dwt_stream.cu) for resolutions of at least 2x2
+                    uint32_t max_ncomp, const ImgComp* img, uint32_t* coef, cudaStream_t st, bool wide = false);
+// register-streaming fast path (dwt_stream.cu) for resolutions of at least 2x2.  img_layout says what img describes:
+// the codec's own image buffer, a caller's memory, or a caller's memory whose first three components are interleaved
+// next to each other (3 or 4 samples per pixel: the colour-transform jobs take the ILV variant)
+enum : uint32_t { IMG_OWN = 0, IMG_CALLER = 1, IMG_CALLER_ILV = 2 };
 void dwt_stream_tiling(uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, bool reversible, bool forward,
                        uint32_t& strips, uint32_t& chunks, uint32_t& chunk_rows, uint32_t& ctas);
 void launch_dwt_fwd_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                           uint32_t ncomp, bool first, uint32_t src_type, const void* image, uint32_t* coef,
-                           cudaStream_t st);
+                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, uint32_t img_layout,
+                           uint32_t* coef, cudaStream_t st);
 void launch_dwt_inv_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                           uint32_t ncomp, bool first, uint32_t src_type, void* image, uint32_t* coef, cudaStream_t st);
+                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, uint32_t img_layout, uint32_t* coef, cudaStream_t st);
 // CTA tiling of a w x h resolution at origin (x0,y0): number of tiles across / down
 void dwt_tiling(uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, uint32_t& tx, uint32_t& ty);
 

@@ -283,7 +283,7 @@ static void region_encode(ojb_shard* s, const void* const* planes, const uint32_
   if (encode_only_upload) { cuda_check(cudaStreamSynchronize(E.stream), "region upload"); return; }
   // 1. this rank's share of the transform and of the block coding
   E.phase = Encoder::PHASE_FRONT;
-  try { E.encode(nullptr, nullptr, true, nullptr, 0, true); } catch (...) { E.phase = Encoder::PHASE_ALL; throw; }
+  try { E.encode(nullptr, nullptr, false, nullptr, 0, true); } catch (...) { E.phase = Encoder::PHASE_ALL; throw; }
   E.phase = Encoder::PHASE_ALL;
   cudaEventRecord(e1, E.stream);
   // 2. how many bytes that made; every rank learns every total
@@ -326,7 +326,7 @@ static void region_encode(ojb_shard* s, const void* const* planes, const uint32_
     const size_t cap = (size_t)sum + (size_t)nb * 24 + E.fixed_blob.size() + E.main_header.size() + (1u << 16);
     s->d_final.reserve(cap + 64);
     E.phase = Encoder::PHASE_BACK;
-    try { total = E.encode(nullptr, nullptr, true, s->d_final.as<uint8_t>(), cap, true); } catch (...) { E.phase = Encoder::PHASE_ALL; throw; }
+    try { total = E.encode(nullptr, nullptr, false, s->d_final.as<uint8_t>(), cap, true); } catch (...) { E.phase = Encoder::PHASE_ALL; throw; }
     E.phase = Encoder::PHASE_ALL;
     if (out) {
       if (total > out_cap) fail(0x000B0030, "output buffer too small: need %zu bytes, have %zu", total, (size_t)out_cap);
@@ -345,7 +345,7 @@ static void region_encode(ojb_shard* s, const void* const* planes, const uint32_
 static void region_decode(ojb_shard* s, uint32_t sample_type, uint32_t writer_rank, void* const* planes, const uint32_t* strides,
                           bool keep_on_device, cudaEvent_t e1) {
   Decoder& D = s->dec; Comm& C = *s->comm;
-  D.decode(nullptr, nullptr, true);
+  D.decode(nullptr, nullptr, false);
   cudaEventRecord(e1, D.stream);
   const Params& P = D.params;
   const uint32_t nc = P.num_comps(), es = esize(sample_type);
@@ -440,7 +440,7 @@ static int shard_encode(ojb_shard* s, const void* const* planes, const uint32_t*
     if (encode_only_upload) { cuda_check(cudaStreamSynchronize(E.stream), "tile upload"); return; }
     // 2. code this rank's tiles: tile-parts, back to back, in device memory
     s->d_parts.reserve(my_in * 2 + (1u << 20));
-    const size_t my_bytes = E.encode(nullptr, nullptr, true, s->d_parts.as<uint8_t>(), s->d_parts.cap, true);
+    const size_t my_bytes = E.encode(nullptr, nullptr, false, s->d_parts.as<uint8_t>(), s->d_parts.cap, true);
     cudaEventRecord(e1, E.stream);
     // 3. sizes: per tile (number of tile-parts, bytes), then the tile-part lengths when a TLM is wanted
     std::vector<uint32_t> mine(2 * ntiles, 0), all((size_t)2 * ntiles * C.world, 0);
@@ -576,7 +576,7 @@ static int shard_decode(ojb_shard* s, const uint8_t* cs, bool cs_on_device, uint
     }
     if (info) { FrameInfo fi; D.info(fi); memcpy(info, &fi, sizeof(fi)); }
     // 3. decode this rank's tiles (result in the device image buffer)
-    D.decode(nullptr, nullptr, true);
+    D.decode(nullptr, nullptr, false);
     cudaEventRecord(e1, D.stream);
     // 4. tile samples to the writer: every tile packed (component after component, tight rows) in a staging buffer
     const Params& P = D.params;
