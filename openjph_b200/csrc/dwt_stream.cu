@@ -468,12 +468,8 @@ __device__ __forceinline__ void fwd_store_pair(const DwtJob& J, const StripGeom&
   }
 }
 
-// TMA = true: the source rows of a strip whose 32 lanes read one contiguous, 16-byte-alignable run of bytes (every
-// interior strip of the usual geometries) are requested by ONE lane with cp.async.bulk (SASS UBLKCP) -- one copy per
-// component row into a row slot of 32 x slot + 16 bytes -- and awaited on an mbarrier per FIFO stage, instead of one
-// cp.async (LDGSTS) per lane; edge strips keep the per-lane requests.  Selected by the host (OJB_DWT_TMA).
 // ILV: the interleaved layout variant (see ilv_issue_row), colour-transform jobs only
-template <bool REV, int NC, int SRC, bool TMA, bool ILV>
+template <bool REV, int NC, int SRC, bool ILV>
 __global__ void __launch_bounds__(DS_WARPS * 32, (REV || NC == 1) ? 5 : 3)
 dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const ImgComp* __restrict__ img,
                       uint32_t* __restrict__ coef)
@@ -482,7 +478,6 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const Img
   constexpr bool FIRSTK = SRC != SRC_COEF;
   __shared__ DwtJob sj;
   __shared__ ImgView sv[FIRSTK ? NC : 1];
-  __shared__ unsigned long long s_bar[TMA ? DS_WARPS * DS_STAGES : 1];
   {
     uint32_t ji = find_job(jobs, njobs, blockIdx.x);
     const uint32_t* s = reinterpret_cast<const uint32_t*>(&jobs[ji]);
@@ -512,52 +507,10 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const Img
   OJB_DYN_SMEM(unsigned char, s_ring);
   // 4 samples in their container (ILV: 4 pixels of up to 4 samples)
   const uint32_t slot = ILV ? 16u * ESK : ((SRC == SRC_U8 || SRC == SRC_U16) ? 8u : 16u);
-  // bulk-copy mode of this strip (warp-uniform): every row of every component starts at the same offset modulo 16
-  bool tma = false;
-  uint32_t skip = 0, c0l0 = 0;
-  if (TMA) {
-    c0l0 = __shfl_sync(0xFFFFFFFFu, (uint32_t)g.c[0], 0);
-    bool ok = g.fast;
-    #pragma unroll
-    for (int k = 0; k < (FIRSTK ? NC : 1); ++k) {
-      const uint32_t off = (FIRSTK ? (uint32_t)(size_t)V[k].org : (uint32_t)J.full_off[0] * 4u) + c0l0 * ESK;
-      const uint32_t pitch = FIRSTK ? (uint32_t)V[k].pitch : J.full_stride[0] * ESK;
-      if (k == 0) skip = off & 15u;
-      ok = ok && (off & 15u) == skip && (pitch & 15u) == 0;
-    }
-    tma = ok;
-  }
   // bytes between the components of a row slot (ILV: samples per pixel, one slot holds them all)
-  const uint32_t cpitch = ILV ? S : (TMA ? 32 * slot + 16 : 32 * slot);
+  const uint32_t cpitch = ILV ? S : 32 * slot;
   const uint32_t row_bytes = ILV ? 32 * slot : NC * cpitch, stage_bytes = 2 * row_bytes;
-  unsigned char* wring = s_ring + (size_t)warp * DS_STAGES * stage_bytes;
-  unsigned char* ring = wring + (size_t)lane * slot + (tma ? skip : 0u);
-  unsigned long long* bar = s_bar + (TMA ? warp * DS_STAGES : 0);
-  if (TMA && tma) {
-    if (lane == 0) { for (int i = 0; i < DS_STAGES; ++i) mbar_init(bar + i, 1); }
-    fence_proxy_async();
-    __syncwarp();
-  }
-  // rows (2 * kk - 1, 2 * kk) of every component into stage `stg`: one bulk copy per component row, lane 0
-  auto issue_tma = [&](int kk, uint32_t stg) {
-    __syncwarp();                                 // the stage's previous rows have been read by every lane
-    if (lane == 0) {
-      fence_proxy_async();
-      const uint32_t nbytes = 32 * slot + 16;
-      mbar_expect_tx(bar + stg, 2u * (FIRSTK ? NC : 1) * nbytes);
-      #pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int vr = reflect_coord(2 * kk - 1 + r, g.y0, g.y1 - 1) - g.y0;
-        #pragma unroll
-        for (int k = 0; k < (FIRSTK ? NC : 1); ++k) {
-          const unsigned char* p = FIRSTK
-            ? V[k].org + ((uint32_t)vr * (uint32_t)V[k].pitch + c0l0 * ESK - skip)
-            : reinterpret_cast<const unsigned char*>(coef) + ((uint32_t)J.full_off[0] * 4u + ((uint32_t)vr * J.full_stride[0] + c0l0) * ESK - skip);
-          bulk_g2s(wring + (size_t)stg * stage_bytes + (size_t)r * row_bytes + (size_t)k * cpitch, p, nbytes, bar + stg);
-        }
-      }
-    }
-  };
+  unsigned char* ring = s_ring + (size_t)warp * DS_STAGES * stage_bytes + (size_t)lane * slot;
 
   // iteration k consumes rows (2k-1, 2k); 5/3 emits the pair (2k-2, 2k-1), 9/7 the pair (2k-4, 2k-3)
   const int k0 = REV ? g.R0 / 2 : g.R0 / 2 - 1;
@@ -565,20 +518,19 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const Img
   T xe[NC][4];                                                // x[2k-2]
   {                                                           // priming row through the last stage
     unsigned char* sp = ring + (size_t)(DS_STAGES - 1) * stage_bytes;
-    fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * k0 - 2, sp - (tma ? skip : 0u), cpitch);     // (per-lane request, old lane layout)
+    fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * k0 - 2, sp, cpitch);
     cp_commit(); cp_wait<0>();
-    fwd_read_row<REV, NC, SRC, ILV>(J, sp - (tma ? skip : 0u), cpitch, xe);
+    fwd_read_row<REV, NC, SRC, ILV>(J, sp, cpitch, xe);
   }
   int issued = k0;
   #pragma unroll
   for (int s = 0; s < DS_STAGES - 1; ++s) {
+    // rows (2 * issued - 1, 2 * issued) into the stage of iteration `issued`.  Both lifting loops repeat this pair:
+    // routed through one lambda or helper, nvcc 12.9 allocates registers differently and the SASS changes
     if (issued <= k1) {
-      if (TMA && tma) issue_tma(issued, (uint32_t)((issued - k0) % DS_STAGES));
-      else {
-        unsigned char* st = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
-        fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, st, cpitch);
-        fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, st + row_bytes, cpitch);
-      }
+      unsigned char* st = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
+      fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, st, cpitch);
+      fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, st + row_bytes, cpitch);
     }
     cp_commit(); ++issued;
   }
@@ -591,8 +543,7 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const Img
       for (int i = 0; i < 4; ++i) hp[c][i] = 0;
     for (int k = k0; k <= k1; ++k) {
       T xo[NC][4], xn[NC][4], lo[NC][4], hi[NC][4];
-      if (TMA && tma) mbar_wait(bar + (k - k0) % DS_STAGES, (uint32_t)(((k - k0) / DS_STAGES) & 1));
-      else cp_wait<DS_STAGES - 2>();
+      cp_wait<DS_STAGES - 2>();
       const unsigned char* st = ring + (size_t)((k - k0) % DS_STAGES) * stage_bytes;
       fwd_read_row<REV, NC, SRC, ILV>(J, st, cpitch, xo);
       fwd_read_row<REV, NC, SRC, ILV>(J, st + row_bytes, cpitch, xn);
@@ -606,12 +557,9 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const Img
           hp[c][i] = (T)h; xe[c][i] = xn[c][i];
         }
       if (issued <= k1) {             // refill the stage consumed one iteration ago
-        if (TMA && tma) issue_tma(issued, (uint32_t)((issued - k0) % DS_STAGES));
-        else {
-          unsigned char* sn = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
-          fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, sn, cpitch);
-          fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, sn + row_bytes, cpitch);
-        }
+        unsigned char* sn = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
+        fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, sn, cpitch);
+        fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, sn + row_bytes, cpitch);
       }
       cp_commit(); ++issued;
       fwd_store_pair<REV, NC>(J, g, coef, 2 * k - 2, lo, hi);      // rows 2k-2 (low), 2k-1 (high)
@@ -625,8 +573,7 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const Img
     const float Kinv = 1.0f / IRV_K;
     for (int k = k0; k <= k1; ++k) {
       T xo[NC][4], xn[NC][4], lo[NC][4], hi[NC][4];
-      if (TMA && tma) mbar_wait(bar + (k - k0) % DS_STAGES, (uint32_t)(((k - k0) / DS_STAGES) & 1));
-      else cp_wait<DS_STAGES - 2>();
+      cp_wait<DS_STAGES - 2>();
       const unsigned char* st = ring + (size_t)((k - k0) % DS_STAGES) * stage_bytes;
       fwd_read_row<REV, NC, SRC, ILV>(J, st, cpitch, xo);
       fwd_read_row<REV, NC, SRC, ILV>(J, st + row_bytes, cpitch, xn);
@@ -642,12 +589,9 @@ dwt_fwd_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const Img
           xe[c][i] = xn[c][i]; d1[c][i] = (T)nd1; s1[c][i] = (T)ns1; d2[c][i] = (T)nd2;
         }
       if (issued <= k1) {
-        if (TMA && tma) issue_tma(issued, (uint32_t)((issued - k0) % DS_STAGES));
-        else {
-          unsigned char* sn = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
-          fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, sn, cpitch);
-          fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, sn + row_bytes, cpitch);
-        }
+        unsigned char* sn = ring + (size_t)((issued - k0) % DS_STAGES) * stage_bytes;
+        fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued - 1, sn, cpitch);
+        fwd_issue_row<NC, SRC, ILV>(J, g, V, coef, 2 * issued, sn + row_bytes, cpitch);
       }
       cp_commit(); ++issued;
       fwd_store_pair<REV, NC>(J, g, coef, 2 * k - 4, lo, hi);      // rows 2k-4 (low), 2k-3 (high)
@@ -962,43 +906,30 @@ dwt_inv_stream_kernel(const DwtJob* __restrict__ jobs, uint32_t njobs, const Img
   }
 }
 
-bool dwt_use_tma() {
-  static const bool v = [] { const char* e = getenv("OJB_DWT_TMA"); return e && atoi(e) != 0; }();
-  return v;
-}
 template <bool REV, int NC, int SRC>
 void launch_fwd(const DwtJob* jobs, uint32_t njobs, uint32_t ctas, const ImgComp* img, uint32_t* coef, cudaStream_t st,
-                uint32_t layout) {
+                bool interleaved) {
   const size_t slot = (SRC == SRC_U8 || SRC == SRC_U16) ? 8 : 16;
   if constexpr (NC == 3 && SRC != SRC_COEF) {
-    if (layout == IMG_CALLER_ILV) {
-      auto k = dwt_fwd_stream_kernel<REV, NC, SRC, false, true>;
+    if (interleaved) {
+      auto k = dwt_fwd_stream_kernel<REV, NC, SRC, true>;
       const size_t smem = (size_t)DS_WARPS * DS_STAGES * 2 * 32 * (4 * slot);     // 16 ES bytes per lane and row
       cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
       return;
     }
   }
-  // bulk-copy staging reads up to 16 bytes past a row's last sample: the codec's own buffer has the slack, a caller's
-  // may not
-  if (dwt_use_tma() && (SRC == SRC_U16 || SRC == SRC_COEF) && (SRC == SRC_COEF || layout == IMG_OWN)) {
-    auto k = dwt_fwd_stream_kernel<REV, NC, SRC, (SRC == SRC_U16 || SRC == SRC_COEF), false>;
-    const size_t smem = (size_t)DS_WARPS * DS_STAGES * 2 * NC * (32 * slot + 16);
-    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
-    return;
-  }
-  auto k = dwt_fwd_stream_kernel<REV, NC, SRC, false, false>;
+  auto k = dwt_fwd_stream_kernel<REV, NC, SRC, false>;
   const size_t smem = (size_t)DS_WARPS * DS_STAGES * 2 * NC * 32 * slot;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
 }
 template <bool REV, int NC, int SRC>
 void launch_inv(const DwtJob* jobs, uint32_t njobs, uint32_t ctas, const ImgComp* img, uint32_t* coef, cudaStream_t st,
-                uint32_t layout) {
+                bool interleaved) {
   const size_t smem = (size_t)DS_WARPS * ((NC == 3) ? DS_STAGES - 1 : DS_STAGES) * NC * 4 * 32 * 8;
   if constexpr (NC == 3 && SRC != SRC_COEF) {
-    if (layout == IMG_CALLER_ILV) {
+    if (interleaved) {
       auto k = dwt_inv_stream_kernel<REV, NC, SRC, true>;
       cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       OJB_LAUNCH(k, dim3(ctas), dim3(DS_WARPS * 32), smem, st, jobs, njobs, img, coef);
@@ -1035,10 +966,10 @@ void dwt_stream_tiling(uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, bool re
 }
 
 void launch_dwt_fwd_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, uint32_t img_layout, uint32_t* coef, cudaStream_t st)
+                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, bool interleaved, uint32_t* coef, cudaStream_t st)
 {
   if (total_ctas == 0) return;
-#define OJB_FWD(REV, NC, SRC) launch_fwd<REV, NC, SRC>(jobs, njobs, total_ctas, img, coef, st, img_layout)
+#define OJB_FWD(REV, NC, SRC) launch_fwd<REV, NC, SRC>(jobs, njobs, total_ctas, img, coef, st, interleaved)
 #define OJB_FWD_SRC(REV, NC) do { if (src_type == SRC_U8) OJB_FWD(REV, NC, SRC_U8); else if (src_type == SRC_U16) OJB_FWD(REV, NC, SRC_U16); \
                                   else OJB_FWD(REV, NC, SRC_I32); } while (0)
   if (reversible) {
@@ -1053,10 +984,10 @@ void launch_dwt_fwd_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ct
 }
 
 void launch_dwt_inv_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, uint32_t img_layout, uint32_t* coef, cudaStream_t st)
+                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, bool interleaved, uint32_t* coef, cudaStream_t st)
 {
   if (total_ctas == 0) return;
-#define OJB_INV(REV, NC, SRC) launch_inv<REV, NC, SRC>(jobs, njobs, total_ctas, img, coef, st, img_layout)
+#define OJB_INV(REV, NC, SRC) launch_inv<REV, NC, SRC>(jobs, njobs, total_ctas, img, coef, st, interleaved)
 #define OJB_INV_SRC(REV, NC) do { if (src_type == SRC_U8) OJB_INV(REV, NC, SRC_U8); else if (src_type == SRC_U16) OJB_INV(REV, NC, SRC_U16); \
                                   else OJB_INV(REV, NC, SRC_I32); } while (0)
   if (reversible) {

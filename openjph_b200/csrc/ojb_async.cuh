@@ -51,32 +51,4 @@ __device__ __forceinline__ void named_bar_arrive(unsigned id, unsigned count) {
 }
 #endif
 
-// ---- TMA bulk copies (cp.async.bulk, SASS UBLKCP) + mbarrier: one elected lane requests a whole contiguous run of
-// global bytes into shared memory; the copy engine completes a transaction count on an mbarrier every reader waits
-// on.  Source, destination and size must be multiples of 16 bytes.
-#ifdef OJB_EMU_BUILD
-__device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned) { *b = 0; }
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long*, unsigned) {}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long*) { memcpy(dst, src, bytes); }
-__device__ __forceinline__ void mbar_wait(unsigned long long*, unsigned) {}
-__device__ __forceinline__ void fence_proxy_async() {}
-#else
-__device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"((unsigned)__cvta_generic_to_shared(b)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* b, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"((unsigned)__cvta_generic_to_shared(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, unsigned long long* b) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               :: "r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src), "r"(bytes), "r"((unsigned)__cvta_generic_to_shared(b)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* b, unsigned parity) {
-  const unsigned a = (unsigned)__cvta_generic_to_shared(b);
-  asm volatile("{\n .reg .pred p;\n WAIT_%=:\n mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n @!p bra WAIT_%=;\n}"
-               :: "r"(a), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-#endif
-
 } // namespace ojb

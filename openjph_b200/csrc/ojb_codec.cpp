@@ -116,12 +116,12 @@ void CodecBase::plan_image(uint32_t sample_type) {
 void CodecBase::use_caller_image(const ImgComp* comps, cudaStream_t caller_stream) {
   const uint32_t nc = params.num_comps(), es = esize_of(img_type);
   memcpy(h_img.p, comps, (size_t)nc * sizeof(ImgComp));
-  caller_layout = IMG_CALLER;
+  caller_interleaved = false;
   if (nc >= 3 && (comps[0].col == 3 || comps[0].col == 4)) {
     bool adj = true;
     for (uint32_t k = 1; k < 3; ++k)
       adj = adj && comps[k].base == comps[0].base + k * es && comps[k].pitch == comps[0].pitch && comps[k].col == comps[0].col;
-    if (adj) caller_layout = IMG_CALLER_ILV;
+    caller_interleaved = adj;
   }
   CK(cudaEventRecord(ev_caller, caller_stream));
   CK(cudaStreamWaitEvent(stream, ev_caller, 0));
@@ -804,7 +804,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     for (const JobGroup& g : jobs[li]) {
       if (g.stream)
         launch_dwt_fwd_stream(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                              g.first, img_type, img_slot(caller_image), caller_image ? caller_layout : (uint32_t)IMG_OWN,
+                              g.first, img_type, img_slot(caller_image), caller_image && caller_interleaved,
                               d_coef.as<uint32_t>(), stream);
       else
         launch_dwt_fwd(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
@@ -866,7 +866,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
       if (attempt == 0 && planes == nullptr && out_on_device && phase == PHASE_ALL)
         run_frame({ (uint64_t)(size_t)dev_out, cap, (uint64_t)nb, (uint64_t)num_fast_blocks, (uint64_t)(size_t)d_slots.p, (uint64_t)(size_t)d_coef.p,
                     rc_frame ? target_bytes : 0, (uint64_t)(size_t)d_rc.p, (uint64_t)(size_t)d_work.p,
-                    (uint64_t)(size_t)img_slot(caller_image), (uint64_t)(caller_image ? caller_layout : (uint32_t)IMG_OWN) }, enqueue_all);
+                    (uint64_t)(size_t)img_slot(caller_image), (uint64_t)(caller_image && caller_interleaved) }, enqueue_all);
       else enqueue_all();
       CK(cudaStreamSynchronize(stream));
       CK(cudaGetLastError());
@@ -1413,7 +1413,7 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool call
     for (const JobGroup& g : jobs[li]) {
       if (g.stream)
         launch_dwt_inv_stream(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                              g.first, img_type, img_slot(caller_image), caller_image ? caller_layout : (uint32_t)IMG_OWN,
+                              g.first, img_type, img_slot(caller_image), caller_image && caller_interleaved,
                               d_coef.as<uint32_t>(), stream);
       else
         launch_dwt_inv(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
@@ -1442,7 +1442,7 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool call
   if (planes == nullptr && dev_cs != nullptr)
     run_frame({ (uint64_t)(size_t)cs_dev, (uint64_t)nb, (uint64_t)(nfast != 0), (uint64_t)(nfast < nb), (uint64_t)cleanup_only, (uint64_t)dec_out,
                 (uint64_t)(size_t)d_scratch.p, (uint64_t)skip_recon, (uint64_t)(size_t)hy, (uint64_t)(size_t)d_coef.p, (uint64_t)(size_t)d_image.p,
-                (uint64_t)(size_t)img_slot(caller_image), (uint64_t)(caller_image ? caller_layout : (uint32_t)IMG_OWN) }, enqueue);
+                (uint64_t)(size_t)img_slot(caller_image), (uint64_t)(caller_image && caller_interleaved) }, enqueue);
   else enqueue();
   CK(cudaStreamSynchronize(stream));
   CK(cudaGetLastError());

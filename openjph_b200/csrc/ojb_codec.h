@@ -81,7 +81,7 @@ public:
   DeviceBuf d_img;
   PinnedBuf h_img;
   cudaEvent_t ev_caller = nullptr;
-  uint32_t caller_layout = IMG_CALLER;   // of the image in slot 1 (IMG_CALLER_ILV: see launch_dwt_fwd_stream)
+  bool caller_interleaved = false;     // the first three components of the image in slot 1 sit next to each other
   const ImgComp* img_slot(bool caller) const { return reinterpret_cast<const ImgComp*>(d_img.p) + (caller ? IMG_SLOTS : 0); }
   // the next frame call reads (encoder) or writes (decoder) the caller's memory described by comps[num_comps], after
   // the work enqueued so far on caller_stream (0: the legacy default stream)

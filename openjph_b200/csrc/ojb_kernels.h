@@ -43,17 +43,16 @@ void launch_dwt_fwd(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, boo
                     uint32_t max_ncomp, const ImgComp* img, uint32_t* coef, cudaStream_t st, bool wide = false);
 void launch_dwt_inv(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
                     uint32_t max_ncomp, const ImgComp* img, uint32_t* coef, cudaStream_t st, bool wide = false);
-// register-streaming fast path (dwt_stream.cu) for resolutions of at least 2x2.  img_layout says what img describes:
-// the codec's own image buffer, a caller's memory, or a caller's memory whose first three components are interleaved
-// next to each other (3 or 4 samples per pixel: the colour-transform jobs take the ILV variant)
-enum : uint32_t { IMG_OWN = 0, IMG_CALLER = 1, IMG_CALLER_ILV = 2 };
+// register-streaming fast path (dwt_stream.cu) for resolutions of at least 2x2.  interleaved: the first three
+// components of the image img describes sit next to each other (3 or 4 samples per pixel: the colour-transform jobs
+// take the ILV variant)
 void dwt_stream_tiling(uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, bool reversible, bool forward,
                        uint32_t& strips, uint32_t& chunks, uint32_t& chunk_rows, uint32_t& ctas);
 void launch_dwt_fwd_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, uint32_t img_layout,
+                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, bool interleaved,
                            uint32_t* coef, cudaStream_t st);
 void launch_dwt_inv_stream(const DwtJob* jobs, uint32_t njobs, uint32_t total_ctas, bool reversible,
-                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, uint32_t img_layout, uint32_t* coef, cudaStream_t st);
+                           uint32_t ncomp, bool first, uint32_t src_type, const ImgComp* img, bool interleaved, uint32_t* coef, cudaStream_t st);
 // CTA tiling of a w x h resolution at origin (x0,y0): number of tiles across / down
 void dwt_tiling(uint32_t x0, uint32_t y0, uint32_t w, uint32_t h, uint32_t& tx, uint32_t& ty);
 

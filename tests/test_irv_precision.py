@@ -86,7 +86,7 @@ BIG_CASES = [
 ALL = dict(CPU_CASES + BIG_CASES)
 # the variant runs (switches read once per process) take this subset
 VARIANT_CASES = ["w121_x1", "w241_x1", "ict_u16_12bit", "levels5_deep", "thin_3x6", "fine_qstep_kmax16", "q90_split"]
-VARIANTS = {"tma": {"OJB_DWT_TMA": "1"}, "no_fast_blocks": {"OJB_NO_FAST_BLOCKS": "1"}}
+VARIANTS = {"no_fast_blocks": {"OJB_NO_FAST_BLOCKS": "1"}}
 
 
 # ---- the streaming DWT's tiling (dwt_stream_tiling, dwt_stream.cu), restated to choose and audit the sizes -------

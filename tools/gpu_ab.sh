@@ -6,25 +6,12 @@ echo "== fast" > gpurun_out/ab.log
 PN=4 python tools/profile_once.py >> gpurun_out/ab.log 2>&1
 echo "== general (OJB_NO_FAST_BLOCKS=1)" >> gpurun_out/ab.log
 OJB_NO_FAST_BLOCKS=1 PN=4 python tools/profile_once.py >> gpurun_out/ab.log 2>&1
-if [ -n "$AB_TMA" ]; then
-echo "== fast, forward DWT rows by cp.async.bulk (OJB_DWT_TMA=1)" >> gpurun_out/ab.log
-for i in 1 2; do OJB_DWT_TMA=1 PN=4 python tools/profile_once.py >> gpurun_out/ab.log 2>&1; done
-echo "== fast, 9/7, OJB_DWT_TMA=1" >> gpurun_out/ab.log
-OJB_DWT_TMA=1 PREV=0 PN=4 python tools/profile_once.py >> gpurun_out/ab.log 2>&1
-echo "== fast again (default staging)" >> gpurun_out/ab.log
-PN=4 python tools/profile_once.py >> gpurun_out/ab.log 2>&1
-fi
 if [ -n "$AB_IRV" ]; then
 echo "== fast, 9/7" >> gpurun_out/ab.log
 PREV=0 PN=4 python tools/profile_once.py >> gpurun_out/ab.log 2>&1
 fi
 timeout 600 ncu --metrics gpu__time_duration.sum,smsp__inst_executed.sum,smsp__issue_active.avg.pct_of_peak_sustained_active,sm__inst_executed_pipe_alu.avg.pct_of_peak_sustained_active,sm__inst_executed_pipe_fma.avg.pct_of_peak_sustained_active,dram__bytes_read.sum,dram__bytes_write.sum \
   --clock-control none -k regex:"ht_|dwt_|gather|assemble" --csv --log-file gpurun_out/ab_ncu.csv python tools/profile_once.py > gpurun_out/ab_ncu.log 2>&1
-if [ -n "$AB_TMA" ]; then
-OJB_DWT_TMA=1 timeout 600 ncu --metrics gpu__time_duration.sum,smsp__inst_executed.sum,smsp__issue_active.avg.pct_of_peak_sustained_active,dram__bytes_read.sum,dram__bytes_write.sum \
-  --clock-control none -k regex:"dwt_fwd" --csv --log-file gpurun_out/ab_ncu_tma.csv python tools/profile_once.py > gpurun_out/ab_ncu_tma.log 2>&1
-grep -E "dwt_fwd" gpurun_out/ab_ncu_tma.csv | grep -E "gpu__time_duration|inst_executed.sum" | cut -d, -f1,5,13- | head -20
-fi
 cat gpurun_out/ab.log
 python - <<'PY'
 import csv
