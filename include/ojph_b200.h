@@ -216,7 +216,7 @@ int ojb_enc_band_info(ojb_encoder* e, uint32_t tile, uint32_t comp, uint32_t res
  * 0x000B0039 the configuration codes 64-bit coefficients, or has a tile-part without packets (both refused by
  * ojb_enc_set_target_size, and by a frame call after a reconfigure to such a configuration);
  * 0x000B003A an internal consistency check: the selection rounds did not end (each round over the target shrinks the
- * selection, so this does not happen). */
+ * selection, so this does not happen); 0x000B0049 the encoder has a target quality (ojb_enc_set_target_mse). */
 int ojb_enc_set_target_size(ojb_encoder* e, uint64_t bytes);
 /* the smallest codestream of the configured geometry: every code-block left out */
 int ojb_enc_min_size(ojb_encoder* e, uint64_t* bytes);
@@ -228,6 +228,49 @@ int ojb_enc_min_size(ojb_encoder* e, uint64_t* bytes);
  * ms4 = distortion, candidate lengths, selection rounds, final block coding */
 int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_t* kmax, uint8_t* k, uint32_t* R,
                       double* D, uint64_t* info5, float* ms4);
+
+/* ---- encode to a target quality ------------------------------------------------------------
+ * With a target mean squared error `mse` (0 = off, the default), every frame call of the encoder returns a codestream
+ * whose squared error against the source is at most floor(mse * N): SSE = the sum over every component c of
+ * sum (decoded - source)^2 over its comp_w x comp_h samples, decoded = what this library's decoder outputs in the
+ * configured sample container (after rounding, clamping and the inverse NLT), N = sum_c comp_w * comp_h.  The stream
+ * is single-layer and cleanup-only, readable by any HTJ2K decoder; each code-block's cleanup pass sits at the
+ * bit-plane a search on the device chose.  Each round of that search reconstructs a selection exactly as the decoder
+ * would and measures its error, so the limit is met exactly; the search stops once the passing and the failing
+ * selection differ by at most max(0.25 %, 64 bytes) of code-block bytes, or their slope keys are adjacent.  A
+ * reversible configuration always reaches the target (key 0 is lossless).  An irreversible one may not: its
+ * quantisation sets a floor, and below it the call returns the unconstrained stream with reached = 0.
+ * Needs, once set, a second coefficient arena and a scratch image of the frame in the configured sample container on
+ * the device (for an 8192 x 8192 x 3 12-bit frame about 1.07 GB, and 0.40 GB in 16-bit or 0.81 GB in 32-bit samples).  After configure.  Not combined with a target size.
+ * Errors: 0x000B0048 mse is negative, infinite or NaN; 0x000B0049 the encoder has a target size (ojb_enc_set_target_size
+ * refuses a size while a quality target is set, with the same code); 0x000B004A the configuration codes 64-bit
+ * coefficients, or has a tile-part without packets (refused here, and by a frame call after a reconfigure to such a
+ * configuration). */
+int ojb_enc_set_target_mse(ojb_encoder* e, double mse);
+#define OJB_QUALITY_MAX_ROUNDS 64
+typedef struct {
+  uint64_t num_samples;          /* N */
+  uint64_t limit;                /* floor(mse * N): the largest SSE accepted */
+  uint64_t sse_lo, sse_hi;       /* exact SSE of the returned stream, 128 bits */
+  double comp_sse[16];           /* the same per component */
+  uint32_t num_comps;
+  uint32_t reached;              /* 1: sse <= limit */
+  uint32_t rounds;               /* measured rounds, and per round: */
+  uint32_t pass_measured;        /* the passing key's selection was measured (0: key 0 of a lossless configuration) */
+  uint64_t round_key[OJB_QUALITY_MAX_ROUNDS];    /* slope key tried (segments with key >= it are taken; 2^32: none) */
+  uint64_t round_sse_lo[OJB_QUALITY_MAX_ROUNDS], round_sse_hi[OJB_QUALITY_MAX_ROUNDS];
+  uint64_t round_body[OJB_QUALITY_MAX_ROUNDS];   /* code-block bytes of the selection */
+  uint64_t pass_key, fail_key;   /* the final bracket: the returned selection, and the failing one (2^32 unmeasured) */
+  uint64_t pass_body, fail_body;
+  uint32_t fail_measured, pad;
+  uint64_t body0;                /* code-block bytes of the unconstrained selection (key 0) */
+  double model_round1;           /* the distortion model's SSE for round 1's selection */
+  float ms_candidates, ms_rounds, ms_final;      /* stage times (CUDA events): distortion + candidate lengths; hull,
+                                                    bracket and rounds; the final block coding */
+  float pad2;
+} ojb_quality_info;
+/* report and parity hook: the search of the last frame encoded with a target quality (0x000B004B: none) */
+int ojb_enc_quality_info(ojb_encoder* e, ojb_quality_info* out);
 
 /* ---- decode: ojph::codestream read side ------------------------------------------------- */
 ojb_decoder* ojb_dec_create(void);

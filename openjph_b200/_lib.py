@@ -65,6 +65,22 @@ class Comment(C.Structure):
     _fields_ = [("data", C.c_void_p), ("len", C.c_uint16), ("rcom", C.c_uint16)]
 
 
+_QR = 64      # OJB_QUALITY_MAX_ROUNDS
+
+
+class QualityInfo(C.Structure):
+    """ojb_quality_info: the quality-target search of the last frame encoded with one"""
+    _fields_ = [
+        ("num_samples", C.c_uint64), ("limit", C.c_uint64), ("sse_lo", C.c_uint64), ("sse_hi", C.c_uint64),
+        ("comp_sse", C.c_double * 16), ("num_comps", C.c_uint32), ("reached", C.c_uint32), ("rounds", C.c_uint32),
+        ("pass_measured", C.c_uint32), ("round_key", C.c_uint64 * _QR), ("round_sse_lo", C.c_uint64 * _QR),
+        ("round_sse_hi", C.c_uint64 * _QR), ("round_body", C.c_uint64 * _QR), ("pass_key", C.c_uint64),
+        ("fail_key", C.c_uint64), ("pass_body", C.c_uint64), ("fail_body", C.c_uint64), ("fail_measured", C.c_uint32),
+        ("pad", C.c_uint32), ("body0", C.c_uint64), ("model_round1", C.c_double), ("ms_candidates", C.c_float), ("ms_rounds", C.c_float),
+        ("ms_final", C.c_float), ("pad2", C.c_float),
+    ]
+
+
 CB_ALLGATHER = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64)
 CB_BCAST = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32)
 CB_SENDRECV = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32)
@@ -112,6 +128,8 @@ SYMBOLS = {
     "ojb_enc_num_blocks": (_U32, [_VP]),
     "ojb_enc_set_target_size": (_I, [_VP, _U64]),
     "ojb_enc_min_size": (_I, [_VP, C.POINTER(_U64)]),
+    "ojb_enc_set_target_mse": (_I, [_VP, C.c_double]),
+    "ojb_enc_quality_info": (_I, [_VP, C.POINTER(QualityInfo)]),
     "ojb_enc_rate_info": (_I, [_VP, C.POINTER(_U32), C.POINTER(_U32), _VP, _VP, _VP, _VP, C.POINTER(_U64), C.POINTER(C.c_float)]),
     "ojb_enc_timings": (None, [_VP, C.POINTER(C.c_float)]),
     "ojb_dec_timings": (None, [_VP, C.POINTER(C.c_float)]),

@@ -158,9 +158,12 @@ class _Base:
 
 
 class Encoder(_Base):
-    def __init__(self, params, sample_type=I32, lib=None, comments=None, target_bytes=None):
+    def __init__(self, params, sample_type=I32, lib=None, comments=None, target_bytes=None, target_mse=None,
+                 target_psnr=None):
         """comments: the extra COM segments of write_headers(file, comments, n): bytes (binary) or str (text);
-        target_bytes: every frame call returns a codestream of at most this many bytes (see set_target_size)"""
+        target_bytes: every frame call returns a codestream of at most this many bytes (see set_target_size);
+        target_mse / target_psnr: every frame call returns a codestream whose decoded error is within this mean squared
+        error / at least this PSNR (see set_target_mse, set_target_psnr)"""
         super().__init__(lib)
         self.h = self.L.ojb_enc_create()
         if not self.h:
@@ -180,6 +183,10 @@ class Encoder(_Base):
         self._out = np.empty(cap, np.uint8)
         if target_bytes:
             self.set_target_size(target_bytes)
+        if target_mse is not None:
+            self.set_target_mse(target_mse)
+        if target_psnr is not None:
+            self.set_target_psnr(target_psnr)
 
     def set_target_size(self, nbytes):
         """cap every following codestream at nbytes (0: no target).  Each code-block is coded at the bit-plane a
@@ -192,6 +199,38 @@ class Encoder(_Base):
         n = C.c_uint64()
         self._check(self.L.ojb_enc_min_size(self.h, C.byref(n)))
         return int(n.value)
+
+    def set_target_mse(self, mse):
+        """bound the decoded error of every following codestream (0: no target): the squared error of the decoded
+        samples against the source, summed over every sample of every component, is at most floor(mse * N), N the
+        number of samples.  The search measures each candidate selection by reconstructing it on the GPU as the decoder
+        would; it returns the smallest stream it finds within the limit.  Below the quantisation floor of an
+        irreversible configuration, the unconstrained stream comes back with quality_info()["reached"] False."""
+        self._check(self.L.ojb_enc_set_target_mse(self.h, float(mse)))
+
+    def set_target_psnr(self, db):
+        """set_target_mse for a PSNR in dB, peak 2^B - 1; every component must have the same bit depth B"""
+        depths = {int(self.params.bit_depth[c]) for c in range(self.params.num_comps)}
+        if len(depths) != 1:
+            raise ValueError("a PSNR target needs one bit depth for every component (have %s)" % sorted(depths))
+        peak = float((1 << depths.pop()) - 1)
+        self.set_target_mse(peak * peak / 10.0 ** (float(db) / 10.0))
+
+    def quality_info(self):
+        """the search of the last frame encoded with a target quality: N, the limit floor(mse * N), the exact squared
+        error of the returned stream (sse, an int) and per component, reached, the rounds (slope key, measured squared
+        error, code-block bytes), the final bracket, the model's prediction for round 1 and the stage times (ms)"""
+        q = _lib.QualityInfo()
+        self._check(self.L.ojb_enc_quality_info(self.h, C.byref(q)))
+        n = q.rounds
+        rounds = [dict(key=int(q.round_key[i]), sse=(int(q.round_sse_hi[i]) << 64) | int(q.round_sse_lo[i]),
+                       body=int(q.round_body[i])) for i in range(n)]
+        return dict(num_samples=int(q.num_samples), limit=int(q.limit), sse=(int(q.sse_hi) << 64) | int(q.sse_lo),
+                    comp_sse=list(q.comp_sse)[:q.num_comps], reached=bool(q.reached), rounds=rounds,
+                    pass_key=int(q.pass_key), fail_key=int(q.fail_key), pass_body=int(q.pass_body),
+                    fail_body=int(q.fail_body), pass_measured=bool(q.pass_measured), fail_measured=bool(q.fail_measured), body0=int(q.body0),
+                    model_round1=float(q.model_round1),
+                    ms=dict(candidates=q.ms_candidates, rounds=q.ms_rounds, final_encode=q.ms_final))
 
     def rate_info(self):
         """the selection of the last frame encoded with a target: K_max, chosen k (k == K_max: left out), R[b, k]

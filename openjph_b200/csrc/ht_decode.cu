@@ -13,6 +13,7 @@
 #include "ojb_device.h"
 #include "ojb_kernels.h"
 #include "ojb_async.cuh"
+#include "dequant.cuh"
 
 namespace ojb {
 
@@ -180,16 +181,6 @@ __device__ __forceinline__ void rev_fill32(RevDec& v) {
   v.unstuff = us;
   v.tmp |= (unsigned long long)t << v.bits;
   v.bits += nb;
-}
-
-__device__ __forceinline__ uint32_t to_output(uint32_t sm, uint32_t mode, uint32_t shift, float delta) {
-  if (mode == DEC_OUT_SIGNMAG) return sm;
-  if (mode == DEC_OUT_INT) {
-    int v = (int)((sm & 0x7FFFFFFFu) >> shift);
-    return (uint32_t)((sm & 0x80000000u) ? -v : v);
-  }
-  float f = __fmul_rn((float)(sm & 0x7FFFFFFFu), delta);
-  return __float_as_uint(f) | (sm & 0x80000000u);
 }
 
 // simple byte-wise readers for the refinement passes

@@ -445,6 +445,33 @@ int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_
     if (ms4) for (int i = 0; i < 4; ++i) ms4[i] = E.rc_ms[i];
   });
 }
+int ojb_enc_set_target_mse(ojb_encoder* e, double mse) {
+  return guarded_on(e->device, [&] {
+    if (!e->configured) fail(0x000B0013, "encoder is not configured");
+    e->enc.set_target_mse(mse);
+  });
+}
+int ojb_enc_quality_info(ojb_encoder* e, ojb_quality_info* out) {
+  return guarded_on(e->device, [&] {
+    Encoder& E = e->enc;
+    if (!e->configured || !E.rq_valid) fail(0x000B004B, "no frame has been encoded with a target quality");
+    const RqState& q = *E.h_rq.as<RqState>();
+    memset(out, 0, sizeof(*out));
+    out->num_samples = E.rq_samples; out->limit = E.rq_limit;
+    out->sse_lo = q.sse_pass[0]; out->sse_hi = q.sse_pass[1];
+    out->num_comps = q.ncomp; out->reached = q.reached;
+    for (uint32_t c = 0; c < q.ncomp && c < 16; ++c) out->comp_sse[c] = (double)q.comp_pass[c][1] * 18446744073709551616.0 + (double)q.comp_pass[c][0];
+    out->rounds = std::min<uint32_t>(q.rounds, OJB_QUALITY_MAX_ROUNDS);
+    for (uint32_t r = 0; r < out->rounds; ++r) {
+      out->round_key[r] = q.round[r].key; out->round_body[r] = q.round[r].body;
+      out->round_sse_lo[r] = q.round[r].sse_lo; out->round_sse_hi[r] = q.round[r].sse_hi;
+    }
+    out->pass_key = q.t_pass; out->fail_key = q.t_fail; out->pass_body = q.body_pass; out->fail_body = q.body_fail;
+    out->pass_measured = q.pass_measured; out->fail_measured = q.fail_measured; out->body0 = q.body0;
+    out->model_round1 = q.model1;
+    out->ms_candidates = E.rq_ms[0]; out->ms_rounds = E.rq_ms[1]; out->ms_final = E.rq_ms[2];
+  });
+}
 void ojb_enc_timings(ojb_encoder* e, float* ms8) {
   for (int i = 0; i < 7; ++i) ms8[i] = e->enc.stage_ms[i];
   ms8[7] = (float)e->enc.host_ms;

@@ -2,6 +2,7 @@
 #include "ojb_codec.h"
 #include "ht_tables.h"
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <chrono>
 #include <atomic>
@@ -108,7 +109,7 @@ void CodecBase::plan_image(uint32_t sample_type) {
     own[c].base = (uint64_t)(size_t)(d_image.as<uint8_t>() + img_off[c]);
     own[c].pitch = (uint64_t)img_w[c] * esize_of(sample_type); own[c].col = 1; own[c].pad = 0;
   }
-  d_img.reserve(2 * IMG_SLOTS * sizeof(ImgComp));
+  d_img.reserve(3 * IMG_SLOTS * sizeof(ImgComp));
   h_img.reserve(IMG_SLOTS * sizeof(ImgComp));
   CK(cudaMemcpy(d_img.p, own.data(), IMG_SLOTS * sizeof(ImgComp), cudaMemcpyHostToDevice));
 }
@@ -286,7 +287,7 @@ void CodecBase::plan_region(bool forward) {
   }
 }
 
-void CodecBase::build_dwt_jobs(bool forward) {
+void CodecBase::build_dwt_jobs(bool forward, std::vector<std::vector<JobGroup>>& jobs, DeviceBuf& d_jobs) {
   const Params& P = params;
   drop_graph(); fgraph.seen.clear();       // a new geometry: whatever was captured launched the old job lists
   if (region.on()) {
@@ -438,7 +439,7 @@ void Encoder::configure(const Params& p, uint32_t sample_type) {
   upload_tables();
   d_coef.reserve((layout.coef_words + 64) * (wide ? 8 : 4));
   CK(cudaMemset(d_coef.p, 0, d_coef.cap));
-  build_dwt_jobs(true);
+  build_dwt_jobs(true, jobs, d_jobs);
   // block descriptors and slots
   h_blocks.assign(layout.num_blocks, EncBlock());
   num_fast_blocks = 0;
@@ -498,6 +499,7 @@ void Encoder::configure(const Params& p, uint32_t sample_type) {
   build_header_plan();
   min_bytes = min_size_of_geometry();
   rc_kc = 0;                           // rate-control tables follow the geometry: planned again on first use
+  rq_planned = false;
   // line-based front end state
   line_cur.assign(params.num_comps(), 0); cur_comp = 0; lines_done = false;
 }
@@ -621,6 +623,7 @@ uint64_t Encoder::min_size_of_geometry() const {
 }
 
 void Encoder::set_target(uint64_t bytes) {
+  if (bytes && rq_on()) fail(0x000B0049, "a target size and a target quality cannot be combined on one encoder");
   if (bytes && wide)
     fail(0x000B0039, "a target size needs the 32-bit coefficient path: this configuration codes 64-bit coefficients");
   if (bytes && !rc_sizing)
@@ -632,6 +635,71 @@ void Encoder::set_target(uint64_t bytes) {
   target_bytes = bytes;
 }
 
+// what a quality target needs of the configuration: the size target's conditions (the selection and the final layout
+// are the same)
+void Encoder::check_target_mse() const {
+  if (wide)
+    fail(0x000B004A, "a target quality needs the 32-bit coefficient path: this configuration codes 64-bit coefficients");
+  if (!rc_sizing)
+    fail(0x000B004A, "a target quality needs every tile-part to hold a packet: the device header plan cannot describe an "
+         "empty tile-part");
+}
+
+void Encoder::set_target_mse(double mse) {
+  if (!(std::isfinite(mse) && mse >= 0.0)) fail(0x000B0048, "the target mean squared error must be a finite number >= 0 (got %g)", mse);
+  if (mse > 0.0 && rc_on()) fail(0x000B0049, "a target size and a target quality cannot be combined on one encoder");
+  if (mse > 0.0) check_target_mse();
+  target_mse = mse;
+  rq_valid = false;
+}
+
+Encoder::~Encoder() {
+  for (cudaEvent_t& e : rq_ev) if (e) { cudaEventDestroy(e); e = nullptr; }
+}
+
+// the buffers of a quality target, after plan_rate_control: the synthesis jobs of the geometry, a second coefficient
+// arena, the scratch image and its descriptors (slot 2), the limit floor(target * N) -- exactly: target = m 2^e with an
+// integer m of at most 53 bits
+void Encoder::plan_quality() {
+  const uint32_t nc = params.num_comps();
+  build_dwt_jobs(false, rq_jobs, d_rq_jobs);
+  d_rcoef.reserve((layout.coef_words + 64) * 4);
+  CK(cudaMemset(d_rcoef.p, 0, d_rcoef.cap));
+  d_rimg.reserve(img_bytes);
+  std::vector<ImgComp> sc(IMG_SLOTS);
+  memset(&rq_image, 0, sizeof(rq_image));
+  rq_image.ncomp = nc; rq_image.sample_type = img_type;
+  rq_samples = 0;
+  for (uint32_t c = 0; c < nc; ++c) {
+    sc[c].base = (uint64_t)(size_t)(d_rimg.as<uint8_t>() + img_off[c]);
+    sc[c].pitch = (uint64_t)img_w[c] * esize_of(img_type); sc[c].col = 1; sc[c].pad = 0;
+    rq_image.w[c] = img_w[c]; rq_image.h[c] = img_h[c];
+    rq_samples += (uint64_t)img_w[c] * img_h[c];
+  }
+  CK(cudaMemcpy(const_cast<ImgComp*>(scratch_slot()), sc.data(), IMG_SLOTS * sizeof(ImgComp), cudaMemcpyHostToDevice));
+  d_rq.reserve(sizeof(RqState));
+  h_rq.reserve(sizeof(RqState));
+  memset(h_rq.p, 0, sizeof(RqState));
+  rc.q = d_rq.as<RqState>();
+  rq_lossless0 = true;
+  for (uint32_t c = 0; c < nc; ++c) rq_lossless0 = rq_lossless0 && params.reversible(c);
+  for (const EncBlock& e : h_blocks) rq_lossless0 = rq_lossless0 && !(e.flags & ENC_CHECK_NEGZERO);
+  for (cudaEvent_t& e : rq_ev) if (!e) CK(cudaEventCreate(&e));
+  rq_planned = true;
+}
+
+// floor(mse * n), exactly (mse = m 2^(e - 53) with an integer m < 2^53), saturated at 2^64 - 1
+static uint64_t sse_limit(double mse, uint64_t n) {
+  int e = 0;
+  const uint64_t m = (uint64_t)std::ldexp(std::frexp(mse, &e), 53);
+  const unsigned __int128 prod = (unsigned __int128)m * n;
+  const int sh = e - 53;
+  if (sh < 0) { const unsigned __int128 v = -sh >= 128 ? 0 : prod >> -sh; return (v >> 64) ? ~0ull : (uint64_t)v; }
+  if (sh >= 64 || (prod && (prod >> (127 - sh)))) return ~0ull;
+  const unsigned __int128 v = prod << sh;
+  return (v >> 64) ? ~0ull : (uint64_t)v;
+}
+
 // per-block weights W_b = G_b C_c s_c^2 and the device tables of the selection (see RcTables)
 void Encoder::plan_rate_control() {
   const uint32_t nb = (uint32_t)h_blocks.size();
@@ -640,6 +708,7 @@ void Encoder::plan_rate_control() {
   const uint32_t kc = kmax + 1;
   std::vector<double> wgt(nb, 0.0);
   std::vector<uint8_t> irv(nb, 0);
+  std::vector<float> dlt(nb, 0.f);
   const Params& P = params;
   const bool ct = P.color_transform();
   std::vector<std::vector<double>> gains(P.num_comps());
@@ -655,13 +724,16 @@ void Encoder::plan_rate_control() {
           const double G = gains[c][P.subband_index(c, rg.res_num, b)];
           const double C = (ct && c < 3) ? colour_weight(!P.reversible(0), c) : 1.0;
           const double s = rev ? 1.0 : (double)P.band_delta(c, rg.res_num, b) * std::ldexp(1.0, (int)P.comps[c].bit_depth);
-          for (uint32_t i = 0; i < bg.nbw * bg.nbh; ++i) { wgt[bg.block_base + i] = G * C * s * s; irv[bg.block_base + i] = rev ? 0 : 1; }
+          for (uint32_t i = 0; i < bg.nbw * bg.nbh; ++i) {
+            wgt[bg.block_base + i] = G * C * s * s; irv[bg.block_base + i] = rev ? 0 : 1; dlt[bg.block_base + i] = bg.delta;
+          }
         }
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 63) & ~(size_t)63; return o; };
   const size_t o_cand = take((size_t)nb * kc * sizeof(EncResult)), o_dist = take((size_t)nb * kc * 8), o_w = take((size_t)nb * 8);
   const size_t o_irv = take(nb), o_nc = take(nb), o_hk = take((size_t)nb * (kc + 1)), o_key = take((size_t)nb * kc * 4);
   const size_t o_len = take((size_t)nb * kc * 4), o_hn = take(nb), o_ch = take(nb), o_st = take(sizeof(RcState));
+  const size_t o_dl = take((size_t)nb * 4);
   d_rc.reserve(off);
   uint8_t* base = d_rc.as<uint8_t>();
   rc.kc = kc;
@@ -670,6 +742,8 @@ void Encoder::plan_rate_control() {
   rc.hull_len = (uint32_t*)(base + o_len); rc.hull_n = base + o_hn; rc.chosen = base + o_ch; rc.state = (RcState*)(base + o_st);
   CK(cudaMemcpy(base + o_w, wgt.data(), (size_t)nb * 8, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(base + o_irv, irv.data(), nb, cudaMemcpyHostToDevice));
+  rc.delta = (const float*)(base + o_dl); rc.q = nullptr;
+  CK(cudaMemcpy(base + o_dl, dlt.data(), (size_t)nb * 4, cudaMemcpyHostToDevice));
   d_work.reserve(std::max<size_t>(1, nb) * sizeof(EncBlock));
   h_rc.reserve(64 + nb);
   rc_kc = kc;
@@ -725,8 +799,15 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   }
   mark(1);
   uint32_t nb = (uint32_t)h_blocks.size();
-  const bool rc_frame = rc_on() && phase == PHASE_ALL && nb > 0;
-  if (rc_frame) {
+  const bool rq_frame = rq_on() && phase == PHASE_ALL && nb > 0;
+  const bool rc_frame = (rc_on() && phase == PHASE_ALL && nb > 0) || rq_frame;
+  if (rq_frame) {
+    check_target_mse();
+    if (rc_kc == 0) plan_rate_control();
+    if (!rq_planned) plan_quality();
+    rq_limit = sse_limit(target_mse, rq_samples);
+    rq_valid = false;
+  } else if (rc_frame) {
     if (wide) fail(0x000B0039, "a target size needs the 32-bit coefficient path: this configuration codes 64-bit coefficients");
     if (target_bytes < min_bytes)
       fail(0x000B0038, "target of %llu bytes is below the smallest codestream of this geometry (%llu bytes)",
@@ -750,6 +831,29 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     launch_ctrl_copy(h_rc.as<uint8_t>() + 64, rc.chosen, nb, stream);
     last_launches += 2;
   };
+  // a round of the quality target: select, reconstruct as the decoder would, synthesise, measure (rate_ctrl.cu)
+  auto rq_round = [&] {
+    launch_rq_select(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), d_coef.as<uint32_t>(), d_rcoef.as<uint32_t>(), rc, stream);
+    last_launches += 3;
+    for (size_t li = rq_jobs.size(); li-- > 0; )
+      for (const JobGroup& g : rq_jobs[li]) {
+        if (g.stream)
+          launch_dwt_inv_stream(d_rq_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
+                                g.first, img_type, scratch_slot(), false, d_rcoef.as<uint32_t>(), stream);
+        else
+          launch_dwt_inv(d_rq_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
+                         scratch_slot(), d_rcoef.as<uint32_t>(), stream, false);
+        ++last_launches;
+      }
+    launch_rq_measure(scratch_slot(), img_slot(caller_image), rq_image, rc, stream);
+    last_launches += 2;
+  };
+  auto rq_final = [&] {
+    launch_rq_final(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
+    launch_ctrl_copy(h_rq.p, rc.q, sizeof(RqState), stream);
+    launch_ctrl_copy(h_rc.as<uint8_t>() + 64, rc.chosen, nb, stream);
+    last_launches += 3;
+  };
   auto enqueue_rc = [&] {
     CK(cudaMemsetAsync(rc.state, 0, sizeof(RcState), stream));
     launch_rc_prepare(d_blocks.as<EncBlock>(), nb, d_coef.as<uint32_t>(), rc, stream);
@@ -759,6 +863,15 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     mark(9);
     launch_rc_hull(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
     last_launches += 4;
+    if (rq_frame) {
+      CK(cudaMemsetAsync(rc.q, 0, sizeof(RqState), stream));
+      launch_rq_init(rc, rq_limit, P.num_comps(), rq_lossless0, stream);
+      ++last_launches;
+      for (int r = 0; r < RQ_GRAPH_ROUNDS; ++r) rq_round();
+      rq_final();
+      mark(10);
+      return;
+    }
     rc_size(true);
     for (int r = 0; r < RC_ROUNDS; ++r) {
       launch_rc_round(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
@@ -770,6 +883,19 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   };
   // after the frame's rounds: the rare selection that still does not fit goes on eagerly; true = it changed
   auto rc_settle = [&]() -> bool {
+    if (rq_frame) {
+      if (h_rq.as<RqState>()->done) return false;
+      CK(cudaEventRecord(rq_ev[0], stream));
+      // the bracket closes within RQ_BODY_ROUNDS + 34 rounds (rq_update_kernel); one synchronisation per round
+      while (!h_rq.as<RqState>()->done) {
+        rq_round();
+        launch_ctrl_copy(h_rq.p, rc.q, sizeof(RqState), stream); ++last_launches;
+        CK(cudaStreamSynchronize(stream));
+      }
+      rq_final();
+      CK(cudaEventRecord(rq_ev[1], stream));
+      return true;
+    }
     if (!rc_frame || h_rc.as<RcState>()->done) return false;
     for (int i = 0; !h_rc.as<RcState>()->done; ++i) {
       // every round over the target strictly lowers the selected body (rc_check_kernel), so there are at most as many
@@ -818,6 +944,16 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   mark(3);
   };
   auto rc_times = [&] {
+    if (rq_frame) {
+      const bool eager = h_rq.as<RqState>()->rounds > (uint32_t)RQ_GRAPH_ROUNDS;
+      cudaEventElapsedTime(&rq_ms[0], ev[2], ev[9]); cudaEventElapsedTime(&rq_ms[1], ev[9], ev[10]);
+      if (eager) {
+        float t = 0; cudaEventElapsedTime(&t, rq_ev[0], rq_ev[1]); rq_ms[1] += t;
+        cudaEventElapsedTime(&rq_ms[2], rq_ev[1], rq_ev[2]);
+      } else cudaEventElapsedTime(&rq_ms[2], ev[10], ev[3]);
+      rq_valid = true;
+      return;
+    }
     if (!rc_frame) return;
     cudaEventElapsedTime(&rc_ms[0], ev[2], ev[8]); cudaEventElapsedTime(&rc_ms[1], ev[8], ev[9]);
     cudaEventElapsedTime(&rc_ms[2], ev[9], ev[10]); cudaEventElapsedTime(&rc_ms[3], ev[10], ev[3]);
@@ -849,7 +985,10 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     for (int attempt = 0; ; ++attempt) {
       auto enqueue_all = [&] {
       if (attempt == 0) { enqueue_front(); launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches; mark(4); mark(5); }
-      else if (recode) { enqueue_code(); launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches; }
+      else if (recode) {
+        enqueue_code(); launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches;
+        if (rq_frame) CK(cudaEventRecord(rq_ev[2], stream));
+      }
       if (fixed_blob.size() <= cap) CK(cudaMemcpyAsync(dev_out, d_fixed.p, fixed_blob.size(), cudaMemcpyDeviceToDevice, stream));
       CK(cudaMemsetAsync(hplan.hscr, 0, hscr_bytes, stream));
       launch_packet_headers(hplan, code_blocks, d_results.as<EncResult>(), wide ? 62u : 30u, fixed_blob.size(), cap,
@@ -866,6 +1005,8 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
       if (attempt == 0 && planes == nullptr && out_on_device && phase == PHASE_ALL)
         run_frame({ (uint64_t)(size_t)dev_out, cap, (uint64_t)nb, (uint64_t)num_fast_blocks, (uint64_t)(size_t)d_slots.p, (uint64_t)(size_t)d_coef.p,
                     rc_frame ? target_bytes : 0, (uint64_t)(size_t)d_rc.p, (uint64_t)(size_t)d_work.p,
+                    rq_frame ? rq_limit : 0, (uint64_t)rq_frame, (uint64_t)(size_t)d_rq.p, (uint64_t)(size_t)d_rcoef.p,
+                    (uint64_t)(size_t)d_rimg.p, (uint64_t)(size_t)d_rq_jobs.p,
                     (uint64_t)(size_t)img_slot(caller_image), (uint64_t)(caller_image && caller_interleaved) }, enqueue_all);
       else enqueue_all();
       CK(cudaStreamSynchronize(stream));
@@ -910,6 +1051,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   if (status_flags & 1u) fail(0x00020005, "block encoder's output slot is full");
   if (rc_settle()) {
     enqueue_code();
+    if (rq_frame) CK(cudaEventRecord(rq_ev[2], stream));
     launch_ctrl_copy(h_results.p, d_results.p, (size_t)nb * sizeof(EncResult), stream); ++last_launches;
     CK(cudaStreamSynchronize(stream));
     CK(cudaGetLastError());
@@ -1213,7 +1355,7 @@ void Decoder::read_headers(const uint8_t* data, size_t len, uint32_t sample_type
 
 void Decoder::setup_geometry(uint32_t sample_type) {
   plan_image(sample_type);
-  build_dwt_jobs(false);
+  build_dwt_jobs(false, jobs, d_jobs);
 }
 
 void Decoder::restrict_resolution(uint32_t skipped_res_for_read, uint32_t skipped_res_for_recon) {

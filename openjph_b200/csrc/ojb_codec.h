@@ -83,6 +83,8 @@ public:
   cudaEvent_t ev_caller = nullptr;
   bool caller_interleaved = false;     // the first three components of the image in slot 1 sit next to each other
   const ImgComp* img_slot(bool caller) const { return reinterpret_cast<const ImgComp*>(d_img.p) + (caller ? IMG_SLOTS : 0); }
+  // slot 2: the encoder's scratch image of a quality target (Encoder::plan_quality)
+  const ImgComp* scratch_slot() const { return reinterpret_cast<const ImgComp*>(d_img.p) + 2 * IMG_SLOTS; }
   // the next frame call reads (encoder) or writes (decoder) the caller's memory described by comps[num_comps], after
   // the work enqueued so far on caller_stream (0: the legacy default stream)
   void use_caller_image(const ImgComp* comps, cudaStream_t caller_stream);
@@ -94,7 +96,8 @@ public:
   struct JobGroup { std::vector<DwtJob> jobs; uint32_t ctas = 0, ncomp = 1; bool first = false, stream = false, reversible = true; size_t dev_off = 0; };
   std::vector<std::vector<JobGroup>> jobs;
   DeviceBuf d_jobs;
-  void build_dwt_jobs(bool forward);
+  // the analysis (forward) or synthesis jobs of the geometry into out, uploaded to dev (the codec's own: jobs, d_jobs)
+  void build_dwt_jobs(bool forward, std::vector<std::vector<JobGroup>>& out, DeviceBuf& dev);
   // one image over several GPUs (ojb_shard.cpp): this object works on the tiles whose mask byte is set (empty =
   // all tiles).  The geometry, arenas and block tables stay those of the whole image, so Isot, canvas coordinates
   // and byte offsets are the single-encoder ones; DWT jobs, code-blocks and packets of the other tiles are skipped.
@@ -125,6 +128,7 @@ public:
 
 class Encoder : public CodecBase {
 public:
+  ~Encoder();
   // finalises parameters, builds geometry and device arenas, produces the main header
   void configure(const Params& p, uint32_t sample_type);
   // encode one frame whose component planes are on the host (pinned or pageable; planes[c] points at sample (0,0) of
@@ -183,6 +187,29 @@ public:
   uint64_t min_size_of_geometry() const;
   void plan_rate_control();
   bool rc_on() const { return target_bytes != 0; }
+  // quality target (rate_ctrl.cu): with a target mean squared error (0 = off), every frame call returns the smallest
+  // stream the search finds whose exact squared error against the source, summed over every sample of every
+  // component, is at most rq_limit = floor(target_mse * N); N = the number of samples.  Each round of the search
+  // reconstructs a selection as the decoder would -- into a second coefficient arena (d_rcoef), through the decoder's
+  // synthesis jobs (rq_jobs) into a scratch image (d_rimg, slot 2 of d_img) -- and measures it.  The buffers exist
+  // only once a target is set (plan_quality)
+  double target_mse = 0;
+  uint64_t rq_limit = 0, rq_samples = 0;
+  bool rq_planned = false, rq_lossless0 = false, rq_valid = false;
+  // rounds inside the frame's graph; a search that needs more goes on eagerly, one synchronisation per round.  Their
+  // inverse DWT launches run even after the search is done.  On the 8K 12-bit frame (H100, tools/quality_probe.py)
+  // searches took 2-13 rounds: four hold the 45 dB 5/3 search and every 9/7 one there
+  enum { RQ_GRAPH_ROUNDS = 4 };
+  std::vector<std::vector<JobGroup>> rq_jobs;
+  DeviceBuf d_rq, d_rcoef, d_rimg, d_rq_jobs;
+  PinnedBuf h_rq;                      // RqState of the last frame
+  RqImage rq_image;
+  cudaEvent_t rq_ev[3] = {nullptr, nullptr, nullptr};
+  float rq_ms[3] = {0, 0, 0};          // last frame: candidates, rounds, final block coding
+  void set_target_mse(double mse);
+  void check_target_mse() const;
+  void plan_quality();
+  bool rq_on() const { return target_mse > 0; }
 };
 
 struct FrameInfo {

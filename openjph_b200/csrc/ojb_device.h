@@ -79,6 +79,27 @@ struct RcState {
   uint32_t rounds;           // selections made (0: the unconstrained stream fits)
   uint32_t pad;
 };
+// the search of a quality target (target squared error): a bracket of slope keys, t_pass (a measured selection whose
+// exact squared error is within the limit; key 0, the unconstrained selection, until one is measured) and t_fail
+// (measured over it; 2^32, every block left out, until one is).  128-bit squared errors as (lo, hi) word pairs.
+#define RQ_MAX_COMPS 16
+#define RQ_MAX_ROUNDS 64
+#define RQ_MODEL_ROUNDS 4          // rounds that may take the model's proposal
+#define RQ_BODY_ROUNDS 16          // rounds that may halve the bracket's body gap; later rounds bisect the key range
+struct RqRound { unsigned long long key, sse_lo, sse_hi, body; };
+struct RqState {
+  unsigned long long limit;                      // floor(target * N)
+  unsigned long long t_pass, t_fail, body_pass, body_fail;
+  unsigned long long sse_pass[2];                // of the selection at t_pass (the one returned)
+  unsigned long long comp_pass[RQ_MAX_COMPS][2]; // per component, of the same selection
+  unsigned long long comp_cur[RQ_MAX_COMPS][2];  // per component, of the selection this round measures
+  unsigned long long key, body;                  // this round's key and body bytes
+  unsigned long long body0;                      // body bytes of the unconstrained selection (key 0)
+  double c;                                      // correction of the model: propose sum_b D_b <= c * limit
+  double model1;                                 // the model's sum_b D_b for the selection of round 1
+  uint32_t rounds, done, reached, pass_measured, fail_measured, force_zero, ncomp, pad;
+  RqRound round[RQ_MAX_ROUNDS];
+};
 // the per-block tables of one frame; kc = 1 + the largest K_max: block b's entries are [b * kc, b * kc + K_max_b]
 struct RcTables {
   uint32_t kc;
@@ -93,7 +114,11 @@ struct RcTables {
   uint8_t* hull_n;           // segments per block
   uint8_t* chosen;           // chosen k per block
   RcState* state;
+  const float* delta;        // the decoder's step per block (DecBlock::delta; irreversible bands)
+  RqState* q;                // quality target only
 };
+// the image planes the quality target compares: component c is comp_w[c] x comp_h[c] samples of the sample container
+struct RqImage { uint32_t ncomp, sample_type, w[RQ_MAX_COMPS], h[RQ_MAX_COMPS]; };
 
 // ---- HT block decoder -------------------------------------------------------------------
 struct DecBlock {

@@ -90,6 +90,14 @@ void launch_rc_hull(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, En
 void launch_rc_round(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res, const RcTables& t, cudaStream_t st);
 void launch_rc_check(const RcTables& t, const uint64_t* total, uint64_t target, uint64_t min_bytes, bool first, cudaStream_t st);
 double colour_weight(bool ict, uint32_t c);
+// quality target (rate_ctrl.cu): the bracket; one round's selection and its reconstruction into the arena `recon`
+// (the decoder's inverse DWT launches then synthesise it); the round's exact squared error and the bracket update;
+// the final selection at t_pass
+void launch_rq_init(const RcTables& t, uint64_t limit, uint32_t ncomp, bool lossless0, cudaStream_t st);
+void launch_rq_select(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res, const uint32_t* coef,
+                      uint32_t* recon, const RcTables& t, cudaStream_t st);
+void launch_rq_measure(const ImgComp* decoded, const ImgComp* source, const RqImage& im, const RcTables& t, cudaStream_t st);
+void launch_rq_final(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res, const RcTables& t, cudaStream_t st);
 // block pieces computed on the device from per-block results + destination offsets
 void launch_gather_blocks(const EncBlock* blocks, const EncResult* results, const uint64_t* dst_off,
                           uint32_t nblocks, const uint8_t* slots, uint8_t* out, cudaStream_t st);
