@@ -223,7 +223,8 @@ int ojb_enc_min_size(ojb_encoder* e, uint64_t* bytes);
 /* parity hook: the selection of the last frame with a target.  *num_blocks, *kc (entries per block: 1 + the largest
  * K_max) always; the arrays when not null: kmax[nb], k[nb] (chosen; k = K_max: left out), R[nb * kc] (cleanup bytes
  * of block b at k, 0xFFFFFFFF: not codable, 0 past the block's top plane), D[nb * kc] (weighted squared error at k,
- * k <= K_max); info5 = final body budget B*, selection rounds, header and marker bytes, codestream bytes, slope-key
+ * k <= K_max; after a transcode kmax[b] is 31 - q_b, q_b the lowest plane the input codes block b down to, and k and
+ * D count planes from q_b); info5 = final body budget B*, selection rounds, header and marker bytes, codestream bytes, slope-key
  * threshold of the final selection (segments with key >= it are taken);
  * ms4 = distortion, candidate lengths, selection rounds, final block coding */
 int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_t* kmax, uint8_t* k, uint32_t* R,
@@ -271,6 +272,38 @@ typedef struct {
 } ojb_quality_info;
 /* report and parity hook: the search of the last frame encoded with a target quality (0x000B004B: none) */
 int ojb_enc_quality_info(ojb_encoder* e, ojb_quality_info* out);
+
+/* ---- transcode a codestream ----------------------------------------------------------------
+ * Re-codes an existing codestream from its decoded code-blocks, never from an image: no inverse or forward transform,
+ * and no second generation of rounding.  The output has the input's geometry and coding parameters and is single-layer
+ * and cleanup-only; its main header is the input's byte for byte without TLM / PLM segments, plus a TLM of its own
+ * when the input had one, and its tile-parts are divided as the input's.  Block b starts at q_b, the lowest plane the
+ * input codes it down to: 30 - missing MSBs with a cleanup pass only, one lower with SigProp / MagRef passes; candidate
+ * k = 0 re-codes exactly the bits the input carried.  So without a target every block is re-coded at k = 0: a stream
+ * this library or OpenJPH wrote comes back byte for byte, and a stream with SigProp / MagRef passes comes back in
+ * cleanup-only form, sample for sample, except that in a block with SigProp but no MagRef pass every sample that
+ * became significant in the cleanup pass keeps its bin centre (a quarter of the cleanup plane's step) as a coded bit.
+ * The encoder's targets apply as to an image: ojb_enc_set_target_size with its min_size and rules, and
+ * ojb_enc_set_target_mse / PSNR, whose source is the input as this library's decoder returns it in the configured
+ * sample container (for a lossless input: the original image).  ojb_enc_rate_info, ojb_enc_quality_info,
+ * ojb_enc_min_size and ojb_enc_timings report on transcodes (timings: [1] the input to the device and its block
+ * decode, [7] the host parse).  The device holds the coefficient arena, block slots, the input and block tables; the
+ * refinement-pass scratch only when the input has such passes; with a target quality also what that target allocates.
+ * Errors: 0x000B004C SOP or EPH markers (Scod bits 1-2), which the output does not write; 0x000B004D a POC, PPM or PPT
+ * segment (packet headers elsewhere or in another order); 0x000B004E a tile-part header segment other than PLT;
+ * 0x000B004F tile-parts that follow none of the divisions the encoder writes (none, by resolution, by component, by
+ * both); 0x000B0050 a configuration on the 64-bit coefficient path (no target size or quality there); 0x000B0051 a
+ * truncated or damaged codestream, or a code-block that fails to decode (there is no resilient transcode);
+ * 0x000B0052 ojb_enc_transcode before ojb_enc_transcode_headers; 0x000B0053 a pixel frame call (encode, upload, raster,
+ * lines) on an encoder configured by ojb_enc_transcode_headers.  A refused input leaves the encoder as it was. */
+/* the encoder counterpart of ojb_dec_read_headers: configures e from a codestream's headers and tile-parts (host
+ * memory, or device memory when on_device, with >= 32 readable bytes after its end); the target setters follow it as
+ * they follow ojb_enc_configure */
+int ojb_enc_transcode_headers(ojb_encoder* e, const void* j2c, uint64_t len, int on_device, uint32_t sample_type);
+/* re-codes the codestream (same main header and tile-part structure as the headers call, else it is read again) to
+ * e's target; out on the device when out_on_device */
+int ojb_enc_transcode(ojb_encoder* e, const void* j2c, uint64_t len, int on_device,
+                      uint8_t* out, uint64_t out_cap, uint64_t* out_len, int out_on_device);
 
 /* ---- decode: ojph::codestream read side ------------------------------------------------- */
 ojb_decoder* ojb_dec_create(void);

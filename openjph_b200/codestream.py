@@ -148,6 +148,22 @@ def comp_dims(p):
             for c in range(p.num_comps)]
 
 
+def _siz_of(head):
+    """(component sizes [(w, h)], bit depths) from a codestream's SIZ segment, which follows SOC"""
+    b = bytes(head)
+    if len(b) < 42 or b[0:4] != b"\xff\x4f\xff\x51":
+        raise OjphError("not a codestream: no SOC and SIZ at its start")
+    u32 = lambda o: int.from_bytes(b[o:o + 4], "big")
+    X, Y, XO, YO = u32(8), u32(12), u32(16), u32(20)
+    nc = int.from_bytes(b[40:42], "big")
+    dims, depths = [], []
+    for c in range(nc):
+        s, dx, dy = b[42 + 3 * c], b[43 + 3 * c], b[44 + 3 * c]
+        dims.append((-(-X // dx) - -(-XO // dx), -(-Y // dy) - -(-YO // dy)))
+        depths.append((s & 0x7F) + 1)
+    return dims, depths
+
+
 class _Base:
     def __init__(self, lib=None):
         self.L = lib if lib is not None else _lib.lib()
@@ -209,12 +225,89 @@ class Encoder(_Base):
         self._check(self.L.ojb_enc_set_target_mse(self.h, float(mse)))
 
     def set_target_psnr(self, db):
-        """set_target_mse for a PSNR in dB, peak 2^B - 1; every component must have the same bit depth B"""
-        depths = {int(self.params.bit_depth[c]) for c in range(self.params.num_comps)}
+        """set_target_mse for a PSNR in dB, peak 2^B - 1; every component must have the same bit depth B (a
+        transcoder takes B from the codestream's headers)"""
+        if self.params is None:
+            depths = set(self._depths)
+        else:
+            depths = {int(self.params.bit_depth[c]) for c in range(self.params.num_comps)}
         if len(depths) != 1:
             raise ValueError("a PSNR target needs one bit depth for every component (have %s)" % sorted(depths))
         peak = float((1 << depths.pop()) - 1)
         self.set_target_mse(peak * peak / 10.0 ** (float(db) / 10.0))
+
+    @classmethod
+    def from_codestream(cls, j2c, sample_type=I32, target_bytes=None, target_mse=None, target_psnr=None, lib=None):
+        """an encoder configured from a codestream's headers and tile-parts (bytes or a uint8 array in host memory, or
+        a 1-D CUDA uint8 tensor), which transcodes: transcode() re-codes such a codestream from its code-blocks,
+        single-layer and cleanup-only, with the input's geometry, coding parameters, main header (less TLM / PLM) and
+        tile-parts, to the targets given here or set later.  The source of a quality target is the input as the
+        Decoder returns it in `sample_type`; target_psnr takes the bit depth from the headers."""
+        self = cls.__new__(cls)
+        _Base.__init__(self, lib)
+        self.h = self.L.ojb_enc_create()
+        if not self.h:
+            raise OjphError(self.L.ojb_last_error().decode(errors="replace"))
+        self.params = None
+        self.sample_type = sample_type
+        ptr, n, dev, head = self._codestream(j2c)
+        self._check(self.L.ojb_enc_transcode_headers(self.h, ptr, n, dev, sample_type))
+        self.dims, self._depths = _siz_of(head)
+        self._out = np.empty(sum(w * h for w, h in self.dims) * 4 + (1 << 20), np.uint8)
+        if target_bytes:
+            self.set_target_size(target_bytes)
+        if target_mse is not None:
+            self.set_target_mse(target_mse)
+        if target_psnr is not None:
+            self.set_target_psnr(target_psnr)
+        return self
+
+    def _codestream(self, j2c):
+        """(address, length, on device, its first bytes) of a codestream in host memory or in a CUDA uint8 tensor"""
+        try:
+            import torch
+            is_tensor = isinstance(j2c, torch.Tensor)
+        except ImportError:
+            is_tensor = False
+        if is_tensor:
+            if not (j2c.is_cuda and j2c.dtype == torch.uint8 and j2c.dim() == 1 and j2c.is_contiguous()):
+                raise ValueError("a codestream tensor is a contiguous 1-D CUDA uint8 tensor")
+            n = j2c.numel()
+            if j2c.untyped_storage().nbytes() - j2c.storage_offset() - n < 32:      # the reader wants 32 bytes of slack
+                pad = torch.zeros(n + 32, dtype=torch.uint8, device=j2c.device)
+                pad[:n].copy_(j2c)
+                j2c = pad[:n]
+            # the headers are read on the host: the bytes must be complete before the call
+            torch.cuda.current_stream(j2c.device).synchronize()
+            self._cs_keep = j2c
+            return j2c.data_ptr(), n, 1, j2c[:min(n, 1 << 16)].cpu().numpy().tobytes()
+        buf = np.frombuffer(j2c, np.uint8) if not isinstance(j2c, np.ndarray) else np.ascontiguousarray(j2c, np.uint8)
+        self._cs_keep = buf
+        return buf.ctypes.data, buf.size, 0, buf[:1 << 16].tobytes()
+
+    def transcode(self, j2c, out=None):
+        """re-code a codestream (see from_codestream) to the encoder's target.  Host bytes / array in: the codestream
+        bytes out.  A CUDA uint8 tensor in: the codestream as a CUDA uint8 tensor, or, with `out` (a CUDA uint8 tensor),
+        written there and its length returned; it never leaves the device.  The call returns with the bytes in place."""
+        ptr, n, dev, _ = self._codestream(j2c)
+        m = C.c_uint64()
+        if not dev:
+            self._check(self.L.ojb_enc_transcode(self.h, ptr, n, 0, self._out.ctypes.data, self._out.size, C.byref(m), 0))
+            return self._out[:m.value].tobytes()
+        import torch
+        where = j2c.device
+        if out is not None:
+            if not (out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous()):
+                raise ValueError("out is a contiguous CUDA uint8 tensor")
+            self._check(self.L.ojb_enc_transcode(self.h, ptr, n, 1, out.data_ptr(), out.numel(), C.byref(m), 1))
+            return int(m.value)
+        stage = getattr(self, "_dev_out", None)
+        if stage is None or stage.device != where:
+            stage = self._dev_out = torch.empty(self._out.size, dtype=torch.uint8, device=where)
+        self._check(self.L.ojb_enc_transcode(self.h, ptr, n, 1, stage.data_ptr(), stage.numel(), C.byref(m), 1))
+        res = torch.empty(m.value + 32, dtype=torch.uint8, device=where)     # 32 readable bytes past the end
+        res[:m.value].copy_(stage[:m.value])
+        return res[:m.value]
 
     def quality_info(self):
         """the search of the last frame encoded with a target quality: N, the limit floor(mse * N), the exact squared

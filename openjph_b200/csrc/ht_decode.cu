@@ -435,7 +435,7 @@ __device__ __forceinline__ void vlc_fill(VlcDec& v) {         // adds 56..64 bit
   vlc_ingest(v, val, 8);
 }
 
-template <int MODE>       // 0: integer output, 1: float output, 2: per-block mode / blocks with refinement passes
+template <int MODE>       // 0: integer output, 1: float output, 2: per-block mode / blocks with refinement passes, 3: DEC_OUT_CODED
 __global__ void __launch_bounds__(DEC1_THREADS)
 ht_decode_serial_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
                         const uint8_t* __restrict__ cs, uint32_t* __restrict__ coef,
@@ -498,6 +498,9 @@ ht_decode_serial_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
   // MODE 0 / 1: the launch has cleanup passes only and one output type, known at compile time
   const uint32_t om = MODE == 0 ? (uint32_t)DEC_OUT_INT : MODE == 1 ? (uint32_t)DEC_OUT_FLOAT
                                 : ((np > 1) ? (uint32_t)DEC_OUT_SIGNMAG : out_mode);
+  // MODE 3: a cleanup-only block drops its bin centre (bit p - 1) at once; a block with refinement passes is decoded
+  // whole, as the passes need the bin centre, and cut below its lowest plane p - 1 afterwards
+  const uint32_t cut = (MODE == 3 && np == 1) ? 1u << (p - 1) : 0u;
   const bool vec4 = ((blk.dst_off | stride) & 3u) == 0;
   const bool narrow = mmsbp2 <= 16;          // m_n <= missing_msbs + 2: the four fields of a quad fit 64 bits
   const uint32_t pscale = 1u << (p - 1);
@@ -621,6 +624,7 @@ ht_decode_serial_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
             uint32_t val;
             if (MODE == 0) { const uint32_t a = mag >> shift; val = a * (1u - 2u * (bits & 1u)); }   // two's complement: +a or -a
             else if (MODE == 1) val = __float_as_uint(__fmul_rn((float)mag, delta)) | (bits << 31);
+            else if (MODE == 3) val = (bits << 31) | (mag - cut);
             else val = to_output((bits << 31) | mag, om, shift, delta);
             o[i][k] = sig ? val : 0u;
           }
@@ -653,7 +657,10 @@ ht_decode_serial_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
 
   if (np > 1) {
     refine_passes(blk, np, data, dst, rec, qstride, p);
-    if (out_mode != DEC_OUT_SIGNMAG)
+    if (MODE == 3)
+      for (uint32_t yy = 0; yy < height; ++yy)
+        for (uint32_t xx = 0; xx < width; ++xx) dst[(size_t)yy * stride + xx] &= ~((1u << (p - 1)) - 1u);
+    else if (out_mode != DEC_OUT_SIGNMAG)
       for (uint32_t yy = 0; yy < height; ++yy)
         for (uint32_t xx = 0; xx < width; ++xx) {
           uint32_t* qp = dst + (size_t)yy * stride + xx;
@@ -686,7 +693,7 @@ ht_decode_serial_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
 // reverse on EMPTY), no polling.  Twice the threads per block: the serial chain of a block -- which bounds the
 // kernel's duration when 49 152 blocks are all that is in flight -- is cut to the longer of the two halves.
 #define SP_BLOCKS 64
-template <int MODE>       // 0: integer output, 1: float output, 2: sign-magnitude
+template <int MODE>       // 0: integer output, 1: float output, 2: sign-magnitude, 3: DEC_OUT_CODED
 __global__ void __launch_bounds__(2 * SP_BLOCKS)
 ht_decode_split_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
                        const uint8_t* __restrict__ cs, uint32_t* __restrict__ coef,
@@ -881,6 +888,7 @@ ht_decode_split_kernel(const DecBlock* __restrict__ blocks, uint32_t nblocks,
             else {
               const uint32_t mag = v * pscale + 2u * pscale;
               if (MODE == 1) val = __float_as_uint(__fmul_rn((float)mag, delta)) | (bits << 31);
+              else if (MODE == 3) val = (bits << 31) | (mag - pscale);     // without the bin centre
               else val = (bits << 31) | mag;
             }
             o[i][k] = sig ? val : 0u;
@@ -1142,12 +1150,13 @@ void launch_ht_decode_serial(const DecBlock* blocks, uint32_t nblocks, uint32_t 
   const size_t smem = (size_t)prev_quads * DEC1_THREADS * sizeof(uint16_t);
   // specialised on the output type when no block carries SigProp / MagRef passes
   auto k = (cleanup_only && out_mode == DEC_OUT_INT) ? ht_decode_serial_kernel<0>
-         : (cleanup_only && out_mode == DEC_OUT_FLOAT) ? ht_decode_serial_kernel<1> : ht_decode_serial_kernel<2>;
+         : (cleanup_only && out_mode == DEC_OUT_FLOAT) ? ht_decode_serial_kernel<1>
+         : out_mode == DEC_OUT_CODED ? ht_decode_serial_kernel<3> : ht_decode_serial_kernel<2>;
   cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   dim3 grid((nblocks + DEC1_THREADS - 1) / DEC1_THREADS), block(DEC1_THREADS);
   if (nfast) {           // blocks flagged DEC_FLAG_FAST (cleanup pass only, one output type): the producer / consumer pair
     auto kf = out_mode == DEC_OUT_INT ? ht_decode_split_kernel<0> : out_mode == DEC_OUT_FLOAT ? ht_decode_split_kernel<1>
-                                                                                            : ht_decode_split_kernel<2>;
+            : out_mode == DEC_OUT_CODED ? ht_decode_split_kernel<3> : ht_decode_split_kernel<2>;
     dim3 g2((nblocks + SP_BLOCKS - 1) / SP_BLOCKS), b2(2 * SP_BLOCKS);
     OJB_LAUNCH(kf, g2, b2, 0, st, blocks, nblocks, codestream, coef, tables, block_status);
   }

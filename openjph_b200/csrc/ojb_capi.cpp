@@ -265,6 +265,7 @@ int ojb_enc_encode_raster(ojb_encoder* e, uint32_t layout, const void* payload, 
   return guarded_on(e->device, [&] {
     if (!e->configured) fail(0x000B0013, "encoder is not configured");
     Encoder& E = e->enc;
+    if (E.transcoding) fail(0x000B0053, "this encoder was configured from a codestream: it transcodes, it has no image");
     uint32_t es = 0; RasterPlanes pl; memset(&pl, 0, sizeof(pl));
     const uint64_t need = raster_geometry(E, layout, es, pl);
     if (payload_bytes != need) fail(0x03000011, "not enough data: the frame takes %llu bytes, got %llu",
@@ -374,12 +375,13 @@ static void read_band(CodecBase& cb, uint32_t tile, uint32_t comp, uint32_t res,
 extern "C" {
 
 void* ojb_enc_device_plane(ojb_encoder* e, uint32_t comp) {
-  if (!e->configured || comp >= e->enc.params.num_comps()) return nullptr;
+  if (!e->configured || e->enc.transcoding || comp >= e->enc.params.num_comps()) return nullptr;
   return img_plane(e->enc, comp);
 }
 int ojb_enc_upload_frame(ojb_encoder* e, const void* const* planes, const uint32_t* strides) {
   return guarded_on(e->device, [&] {
     if (!e->configured) fail(0x000B0013, "encoder is not configured");
+    if (e->enc.transcoding) fail(0x000B0053, "this encoder was configured from a codestream: it transcodes, it has no image");
     upload_frame(e->enc, planes, strides);
   });
 }
@@ -420,7 +422,14 @@ int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_
     const uint32_t nb = (uint32_t)E.h_blocks.size(), n = E.rc_kc;
     *num_blocks = nb; *kc = n;
     const RcTables& t = E.rc;
-    if (kmax) for (uint32_t b = 0; b < nb; ++b) kmax[b] = (uint8_t)(31u - E.h_blocks[b].p);
+    // where each block's candidates start: 31 - K_max, or for a transcode the input's lowest coded plane q_b
+    std::vector<EncBlock> xb;
+    if (E.transcoding && nb) {
+      xb.resize(nb);
+      cuda_check(cudaMemcpy(xb.data(), E.d_xblocks.p, (size_t)nb * sizeof(EncBlock), cudaMemcpyDeviceToHost), "rate_info");
+    }
+    const EncBlock* blk = xb.empty() ? E.h_blocks.data() : xb.data();
+    if (kmax) for (uint32_t b = 0; b < nb; ++b) kmax[b] = (uint8_t)(31u - blk[b].p);
     if (k) cuda_check(cudaMemcpy(k, t.chosen, nb, cudaMemcpyDeviceToHost), "rate_info");
     if (R) {
       std::vector<EncResult> c((size_t)nb * n); std::vector<uint8_t> nc(nb);
@@ -435,7 +444,7 @@ int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_
     if (D) {
       cuda_check(cudaMemcpy(D, t.dist, (size_t)nb * n * 8, cudaMemcpyDeviceToHost), "rate_info");
       for (uint32_t b = 0; b < nb; ++b)
-        for (uint32_t j = 32u - E.h_blocks[b].p; j < n; ++j) D[(size_t)b * n + j] = 0.0;     // past K_max: not computed
+        for (uint32_t j = 32u - blk[b].p; j < n; ++j) D[(size_t)b * n + j] = 0.0;     // past K_max: not computed
     }
     if (info5) {
       RcState s; cuda_check(cudaMemcpy(&s, t.state, sizeof(s), cudaMemcpyDeviceToHost), "rate_info");
@@ -443,6 +452,21 @@ int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_
       info5[4] = s.thresh == 0xFFFFFFFFu ? (1ull << 32) : s.thresh;
     }
     if (ms4) for (int i = 0; i < 4; ++i) ms4[i] = E.rc_ms[i];
+  });
+}
+int ojb_enc_transcode_headers(ojb_encoder* e, const void* j2c, uint64_t len, int on_device, uint32_t sample_type) {
+  return guarded_on(e->device, [&] {
+    if (sample_type > 2) fail(0x000B0012, "unknown sample container");
+    e->configured = false;               // a failing call leaves no half-built encoder behind
+    e->enc.transcode_headers(static_cast<const uint8_t*>(j2c), (size_t)len, on_device != 0, sample_type);
+    e->configured = true;
+  });
+}
+int ojb_enc_transcode(ojb_encoder* e, const void* j2c, uint64_t len, int on_device,
+                      uint8_t* out, uint64_t out_cap, uint64_t* out_len, int out_on_device) {
+  return guarded_on(e->device, [&] {
+    *out_len = e->enc.transcode(static_cast<const uint8_t*>(j2c), (size_t)len, on_device != 0, out, (size_t)out_cap,
+                                out_on_device != 0);
   });
 }
 int ojb_enc_set_target_mse(ojb_encoder* e, double mse) {

@@ -80,7 +80,7 @@ void CodecBase::upload_tables() {
 
 static inline uint32_t esize_of(uint32_t st) { return st == ST_U8 ? 1u : (st == ST_U16 ? 2u : 4u); }
 
-void CodecBase::plan_image(uint32_t sample_type) {
+void CodecBase::plan_image(uint32_t sample_type, bool alloc) {
   img_type = sample_type;
   uint32_t nc = params.num_comps();
   img_off.assign(nc, 0); img_w.assign(nc, 0); img_h.assign(nc, 0);
@@ -102,11 +102,11 @@ void CodecBase::plan_image(uint32_t sample_type) {
     off = (off + 255) & ~(size_t)255;
   }
   img_bytes = off + 256;
-  d_image.reserve(img_bytes);
+  if (alloc) d_image.reserve(img_bytes);
   if (nc > IMG_SLOTS) fail(0x000B0008, "%u components: the frame interface carries at most %u", nc, (uint32_t)IMG_SLOTS);
   std::vector<ImgComp> own(IMG_SLOTS);
   for (uint32_t c = 0; c < nc; ++c) {
-    own[c].base = (uint64_t)(size_t)(d_image.as<uint8_t>() + img_off[c]);
+    own[c].base = alloc ? (uint64_t)(size_t)(d_image.as<uint8_t>() + img_off[c]) : 0;
     own[c].pitch = (uint64_t)img_w[c] * esize_of(sample_type); own[c].col = 1; own[c].pad = 0;
   }
   d_img.reserve(3 * IMG_SLOTS * sizeof(ImgComp));
@@ -431,11 +431,18 @@ static uint32_t widest_block(const Layout& L) {
 void Encoder::configure(const Params& p, uint32_t sample_type) {
   params = p;
   params.finalize_for_encode();
+  transcoding = false;
+  main_header.clear();
+  params.write_main_header(main_header, nullptr, nullptr, 0);
+  setup(sample_type);
+}
+
+void Encoder::setup(uint32_t sample_type) {
   wide = params.needs_wide();
   if (wide && sample_type != ST_I32) fail(0x000B0010, "samples beyond 16 bits need the 32-bit sample container");
   layout.build(params);
   max_block_w = widest_block(layout);
-  plan_image(sample_type);
+  plan_image(sample_type, !transcoding);            // a transcoder needs an image only for a quality target (plan_quality)
   upload_tables();
   d_coef.reserve((layout.coef_words + 64) * (wide ? 8 : 4));
   CK(cudaMemset(d_coef.p, 0, d_coef.cap));
@@ -494,8 +501,7 @@ void Encoder::configure(const Params& p, uint32_t sample_type) {
   h_dst.reserve(std::max<size_t>(1, h_blocks.size()) * 8);
   d_status.reserve(256); h_status.reserve(256);
   coded.assign(layout.num_blocks, CodedBlock());
-  main_header.clear();
-  params.write_main_header(main_header, nullptr, nullptr, 0);
+  if (transcoding) d_xblocks.reserve(std::max<size_t>(1, h_blocks.size()) * sizeof(EncBlock));
   build_header_plan();
   min_bytes = min_size_of_geometry();
   rc_kc = 0;                           // rate-control tables follow the geometry: planned again on first use
@@ -662,6 +668,7 @@ Encoder::~Encoder() {
 // integer m of at most 53 bits
 void Encoder::plan_quality() {
   const uint32_t nc = params.num_comps();
+  if (transcoding) plan_image(img_type, true);     // the source: the input as the decoder returns it
   build_dwt_jobs(false, rq_jobs, d_rq_jobs);
   d_rcoef.reserve((layout.coef_words + 64) * 4);
   CK(cudaMemset(d_rcoef.p, 0, d_rcoef.cap));
@@ -782,6 +789,8 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
 {
   const Params& P = params;
   uint32_t nc = P.num_comps(), es = esize_of(img_type);
+  if (transcoding && phase != PHASE_TRANSCODE)
+    fail(0x000B0053, "this encoder was configured from a codestream (ojb_enc_transcode_headers): it transcodes, it has no image");
   last_launches = 0;
   mark(0);
   // 1. image planes -> device
@@ -799,8 +808,9 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   }
   mark(1);
   uint32_t nb = (uint32_t)h_blocks.size();
-  const bool rq_frame = rq_on() && phase == PHASE_ALL && nb > 0;
-  const bool rc_frame = (rc_on() && phase == PHASE_ALL && nb > 0) || rq_frame;
+  const bool whole = phase == PHASE_ALL || phase == PHASE_TRANSCODE;
+  const bool rq_frame = rq_on() && whole && nb > 0;
+  const bool rc_frame = (rc_on() && whole && nb > 0) || rq_frame;
   if (rq_frame) {
     check_target_mse();
     if (rc_kc == 0) plan_rate_control();
@@ -820,7 +830,8 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   // rate control: the candidates and the rounds of the selection (rate_ctrl.cu); each round sizes its selection with the
   // packet header kernels, so the block coder's final pass and the headers see the chosen planes in d_work
   EncBlock* const work = d_work.as<EncBlock>();
-  const EncBlock* const code_blocks = rc_frame ? work : d_blocks.as<EncBlock>();
+  const EncBlock* const blocks = frame_blocks();          // where each block starts (a transcode: at the input's plane)
+  const EncBlock* const code_blocks = rc_frame ? work : blocks;
   auto rc_size = [&](bool first) {
     launch_packet_header_total(hplan, work, d_results.as<EncResult>(), 30u, fixed_blob.size(), true, stream);
     launch_rc_check(rc, hplan.total, target_bytes, min_bytes, first, stream);
@@ -833,7 +844,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   };
   // a round of the quality target: select, reconstruct as the decoder would, synthesise, measure (rate_ctrl.cu)
   auto rq_round = [&] {
-    launch_rq_select(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), d_coef.as<uint32_t>(), d_rcoef.as<uint32_t>(), rc, stream);
+    launch_rq_select(d_blocks.as<EncBlock>(), blocks, nb, work, d_results.as<EncResult>(), d_coef.as<uint32_t>(), d_rcoef.as<uint32_t>(), rc, stream);
     last_launches += 3;
     for (size_t li = rq_jobs.size(); li-- > 0; )
       for (const JobGroup& g : rq_jobs[li]) {
@@ -849,23 +860,23 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     last_launches += 2;
   };
   auto rq_final = [&] {
-    launch_rq_final(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
+    launch_rq_final(blocks, nb, work, d_results.as<EncResult>(), rc, stream);
     launch_ctrl_copy(h_rq.p, rc.q, sizeof(RqState), stream);
     launch_ctrl_copy(h_rc.as<uint8_t>() + 64, rc.chosen, nb, stream);
     last_launches += 3;
   };
   auto enqueue_rc = [&] {
     CK(cudaMemsetAsync(rc.state, 0, sizeof(RcState), stream));
-    launch_rc_prepare(d_blocks.as<EncBlock>(), nb, d_coef.as<uint32_t>(), rc, stream);
+    launch_rc_prepare(blocks, nb, d_coef.as<uint32_t>(), rc, stream);
     mark(8);
-    launch_ht_encode_lengths(d_blocks.as<EncBlock>(), nb, rc.kc, rc.ncand, max_block_w, d_coef.as<uint32_t>(), rc.cand,
+    launch_ht_encode_lengths(blocks, nb, rc.kc, rc.ncand, max_block_w, d_coef.as<uint32_t>(), rc.cand,
                              d_tables_enc.as<uint16_t>(), stream);
     mark(9);
-    launch_rc_hull(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
+    launch_rc_hull(blocks, nb, work, d_results.as<EncResult>(), rc, stream);
     last_launches += 4;
     if (rq_frame) {
       CK(cudaMemsetAsync(rc.q, 0, sizeof(RqState), stream));
-      launch_rq_init(rc, rq_limit, P.num_comps(), rq_lossless0, stream);
+      launch_rq_init(rc, rq_limit, P.num_comps(), rq_lossless0 && !(phase == PHASE_TRANSCODE && xc_two_pass), stream);
       ++last_launches;
       for (int r = 0; r < RQ_GRAPH_ROUNDS; ++r) rq_round();
       rq_final();
@@ -874,7 +885,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     }
     rc_size(true);
     for (int r = 0; r < RC_ROUNDS; ++r) {
-      launch_rc_round(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
+      launch_rc_round(blocks, nb, work, d_results.as<EncResult>(), rc, stream);
       last_launches += 2;
       rc_size(false);
     }
@@ -902,7 +913,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
       // rounds as distinct selections: one more hull segment per block and round at the very worst
       if ((uint64_t)i > (uint64_t)nb * rc.kc + 2)
         fail(0x000B003A, "rate control did not settle on a selection that fits the target (internal error)");
-      launch_rc_round(d_blocks.as<EncBlock>(), nb, work, d_results.as<EncResult>(), rc, stream);
+      launch_rc_round(blocks, nb, work, d_results.as<EncResult>(), rc, stream);
       last_launches += 2;
       rc_size(false);
       rc_state_out();
@@ -925,7 +936,8 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   auto enqueue_front = [&] {
   CK(cudaMemsetAsync(d_status.p, 0, 16, stream));
   if (caller_image) enqueue_caller_image();
-  if (phase != PHASE_BACK)
+  if (phase == PHASE_TRANSCODE) enqueue_transcode_front();
+  else if (phase != PHASE_BACK)
   for (size_t li = 0; li < jobs.size(); ++li)
     for (const JobGroup& g : jobs[li]) {
       if (g.stream)
@@ -1060,12 +1072,18 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   // 3. packet headers and final layout on the host (with a target: at the planes the selection chose)
   const EncResult* res = h_results.as<EncResult>();
   const uint8_t* chosen = rc_frame ? h_rc.as<uint8_t>() + 64 : nullptr;
+  std::vector<EncBlock> xb;                // a transcode's per-frame start planes
+  if (phase == PHASE_TRANSCODE && nb) {
+    xb.resize(nb);
+    CK(cudaMemcpy(xb.data(), d_xblocks.p, (size_t)nb * sizeof(EncBlock), cudaMemcpyDeviceToHost));
+  }
+  const EncBlock* hb = xb.empty() ? h_blocks.data() : xb.data();
   for (uint32_t b = 0; b < nb; ++b) {
     CodedBlock& cb = coded[b];
     uint32_t len = res[b].len_head + res[b].len_tail;
     cb.pass_len[0] = len; cb.pass_len[1] = 0;
     cb.num_passes = len ? 1 : 0;
-    cb.missing_msbs = len ? (uint8_t)((wide ? 62u : 30u) - h_blocks[b].p - (chosen ? chosen[b] : 0u)) : 0;
+    cb.missing_msbs = len ? (uint8_t)((wide ? 62u : 30u) - hb[b].p - (chosen ? chosen[b] : 0u)) : 0;
   }
   struct Pkt { PacketRef ref; std::vector<uint8_t> hdr; uint32_t hdr_len, body; };
   struct TilePart { uint32_t tile, first, count, tp_idx, tp_cnt; uint64_t bytes; };
@@ -1299,8 +1317,10 @@ void Decoder::read_headers(const uint8_t* data, size_t len, uint32_t sample_type
   layout.build(params);
   max_block_w = widest_block(layout);
   upload_tables();
-  d_coef.reserve((layout.coef_words + 64) * (wide ? 8 : 4));
-  setup_geometry(sample_type);
+  if (!parse_only) {
+    d_coef.reserve((layout.coef_words + 64) * (wide ? 8 : 4));
+    setup_geometry(sample_type);
+  }
   // geometry part of the block records
   h_dec_proto.assign(layout.num_blocks, DecBlock());
   block_res.assign(layout.num_blocks, 0);
@@ -1331,7 +1351,8 @@ void Decoder::read_headers(const uint8_t* data, size_t len, uint32_t sample_type
               scratch += (size_t)qs * nqr;
             }
         }
-  d_scratch.reserve((scratch + 64) * 4);
+  scratch_words = scratch;
+  if (!parse_only) d_scratch.reserve((scratch + 64) * 4);
   coded.assign(layout.num_blocks, CodedBlock());
   block_static.assign(layout.num_blocks, DecStatic());
   for (size_t b = 0; b < h_dec_proto.size(); ++b) {
@@ -1401,6 +1422,8 @@ void Decoder::parse_tiles() {
   std::vector<std::vector<PacketRef>> seqs(ntiles);
   std::vector<uint32_t> next_pkt(ntiles, 0), next_tp(ntiles, 0);
   std::vector<bool> have_seq(ntiles, false);
+  tp_starts.assign(ntiles, std::vector<uint32_t>());
+  tp_segments = 0;
   size_t pos = first_sot;
   const uint8_t* d = j2c;
   HostMirror* hm = mirrored ? &mirror : nullptr;
@@ -1437,6 +1460,7 @@ void Decoder::parse_tiles() {
       bool seg = (m == 0x52 || m == 0x53 || m == 0x5C || m == 0x5D || m == 0x5E || m == 0x5F || m == 0x61 ||
                   m == 0x58 || m == 0x64 || m == 0x76);
       if (!seg) { ++q; continue; }
+      tp_segments |= (m == 0x61 || m == 0x5F) ? 2u : (m != 0x58 ? 1u : 0u);
       if (q + 4 > tp_end) break;
       uint32_t L = ((uint32_t)d[q + 2] << 8) | d[q + 3];
       q += 2 + L;
@@ -1453,6 +1477,7 @@ void Decoder::parse_tiles() {
     uint32_t payload = Psot ? Psot - 12 : (uint32_t)(j2c_len - tile_start);
     uint32_t data_left = payload - (uint32_t)(q - tile_start);     // what Psot promises, not what the buffer holds
     if (!have_seq[Isot]) { std::vector<uint32_t> tpf; layout.packet_sequence(Isot, seqs[Isot], tpf); have_seq[Isot] = true; }
+    tp_starts[Isot].push_back(next_pkt[Isot]);
     try {
       std::vector<PacketRef>& seq = seqs[Isot];
       while (data_left > 0 && next_pkt[Isot] < seq.size()) {
@@ -1465,6 +1490,57 @@ void Decoder::parse_tiles() {
     }
     pos = tp_end;
   }
+  pkts_read = next_pkt;
+}
+
+// the frame's part of every block record (the geometry part sits in d_proto): lengths, passes, missing msbs, where
+// the bytes are, and whether the block goes through the specialised kernel (one output type per launch).
+// (the geometry a block's record needs here -- static flags, whether its shape suits the specialised kernel --
+// sits in 4 bytes per block, block_static, instead of the 48-byte DecBlock prototype)
+BlockFrame Decoder::frame_records(uint32_t dec_out, DecDyn* hy) {
+  BlockFrame f; f.dec_out = dec_out;
+  const uint32_t nb = (uint32_t)h_dec_proto.size();
+  const bool fast_ok = dec_out != DEC_OUT_PER_BLOCK && !no_fast_blocks && !wide;
+  const bool masked = !block_wanted.empty(), restricted = skip_read > 0;
+  const DecStatic* bst = block_static.data();
+  for (uint32_t b = 0; b < nb; ++b) {
+    const CodedBlock& cb = coded[b];
+    const DecStatic g = bst[b];
+    uint32_t len1 = cb.pass_len[0], len2 = cb.pass_len[1], np = cb.num_passes;
+    const uint32_t mm = cb.missing_msbs;
+    bool skip = false;
+    if (masked && !block_wanted[b]) { np = 0; len1 = len2 = 0; skip = true; }   // another rank's tile / rows
+    if (restricted && block_res[b] < skip_read) {            // resolution not read: its bands are zero ...
+      np = 0; len1 = len2 = 0;
+      if (block_res[b] < skip_recon) skip = true;            // ... and not even needed: nothing to fill
+    }
+    if (np > 1) f.cleanup_only = false;
+    uint32_t flags = g.flags;
+    // dec_block_is_fast(): the shape part is g.fast_shape, the frame's part is checked here
+    if (fast_ok && g.fast_shape && !skip && np == 1 && len1 >= 2 && mm + 2u <= 16u && g.K_max > mm) { flags |= DEC_FLAG_FAST; ++f.nfast; }
+    DecDyn y; y.data_off = cb.data_off; y.len1 = (uint16_t)len1; y.len2 = (uint16_t)len2;
+    y.num_passes = (uint8_t)np; y.missing_msbs = (uint8_t)mm; y.flags = (uint8_t)flags; y.skip = skip ? 1 : 0;
+    hy[b] = y;
+  }
+  return f;
+}
+
+// the block decoders of one frame into the arena coef: records merged from hy, then the kernels (launches counted)
+void Decoder::enqueue_blocks(const BlockFrame& f, const DecDyn* hy, const uint8_t* cs, uint32_t* coef, cudaStream_t st,
+                             const SideStream* sd, uint32_t& launches) {
+  const uint32_t nb = (uint32_t)h_dec_proto.size();
+  if (nb) { launch_dec_merge(d_dec.as<DecBlock>(), d_proto.as<DecBlock>(), hy, nb, st); ++launches; }
+  if (wide) {
+    if (!f.cleanup_only) fail(0x000B0009, "SigProp / MagRef passes are not implemented on the 64-bit coefficient path");
+    launch_ht_decode_wide(d_dec.as<DecBlock>(), nb, max_block_w, cs, coef, d_tables_dec.as<uint16_t>(), false,
+                          d_bstatus.as<uint32_t>(), st);
+  } else {
+    if (!f.cleanup_only) d_scratch.reserve((scratch_words + 64) * 4);
+    launch_ht_decode_serial(d_dec.as<DecBlock>(), nb, f.nfast, max_block_w, cs, coef, d_scratch.as<uint32_t>(),
+                            d_tables_dec.as<uint16_t>(), f.dec_out, f.cleanup_only,
+                            d_bstatus.as<uint32_t>(), st, sd);
+  }
+  launches += 1 + (f.nfast ? 1 : 0) + (f.nfast < nb ? 1 : 0);
 }
 
 uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool caller_image) {
@@ -1504,49 +1580,14 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool call
   }
   uint32_t nb = (uint32_t)h_dec_proto.size();
   DecDyn* hy = h_dyn.as<DecDyn>();
-  uint32_t nfast = 0;
-  bool cleanup_only = true;                 // lets the block decoder be specialised
-  const uint32_t dec_out = (any_rev_blocks && any_irv_blocks) ? (uint32_t)DEC_OUT_PER_BLOCK : any_irv_blocks ? (uint32_t)DEC_OUT_FLOAT : (uint32_t)DEC_OUT_INT;
-  const bool fast_ok = dec_out != DEC_OUT_PER_BLOCK && !no_fast_blocks && !wide;
-  // the frame's part of every block record (the geometry part sits in d_proto): lengths, passes, missing msbs, where
-  // the bytes are, and whether the block goes through the specialised kernel (one output type per launch).
-  // (the geometry a block's record needs here -- static flags, whether its shape suits the specialised kernel --
-  // sits in 4 bytes per block, block_static, instead of the 48-byte DecBlock prototype)
-  const bool masked = !block_wanted.empty(), restricted = skip_read > 0;
-  const DecStatic* bst = block_static.data();
-  for (uint32_t b = 0; b < nb; ++b) {
-    const CodedBlock& cb = coded[b];
-    const DecStatic g = bst[b];
-    uint32_t len1 = cb.pass_len[0], len2 = cb.pass_len[1], np = cb.num_passes;
-    const uint32_t mm = cb.missing_msbs;
-    bool skip = false;
-    if (masked && !block_wanted[b]) { np = 0; len1 = len2 = 0; skip = true; }   // another rank's tile / rows
-    if (restricted && block_res[b] < skip_read) {            // resolution not read: its bands are zero ...
-      np = 0; len1 = len2 = 0;
-      if (block_res[b] < skip_recon) skip = true;            // ... and not even needed: nothing to fill
-    }
-    if (np > 1) cleanup_only = false;
-    uint32_t flags = g.flags;
-    // dec_block_is_fast(): the shape part is g.fast_shape, the frame's part is checked here
-    if (fast_ok && g.fast_shape && !skip && np == 1 && len1 >= 2 && mm + 2u <= 16u && g.K_max > mm) { flags |= DEC_FLAG_FAST; ++nfast; }
-    DecDyn y; y.data_off = cb.data_off; y.len1 = (uint16_t)len1; y.len2 = (uint16_t)len2;
-    y.num_passes = (uint8_t)np; y.missing_msbs = (uint8_t)mm; y.flags = (uint8_t)flags; y.skip = skip ? 1 : 0;
-    hy[b] = y;
-  }
+  const BlockFrame bf = frame_records(native_out(), hy);
+  const uint32_t nfast = bf.nfast, dec_out = bf.dec_out;
+  const bool cleanup_only = bf.cleanup_only;
   host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
   if (getenv("OJB_PARSE_PROF")) fprintf(stderr, "decode host: parse %.3f ms, records %.3f ms\n", std::chrono::duration<double, std::milli>(host_t1 - host_t0).count(), host_ms - std::chrono::duration<double, std::milli>(host_t1 - host_t0).count());
   auto enqueue = [&] {
   mark(2);
-  if (nb) { launch_dec_merge(d_dec.as<DecBlock>(), d_proto.as<DecBlock>(), hy, nb, stream); ++last_launches; }
-  if (wide) {
-    if (!cleanup_only) fail(0x000B0009, "SigProp / MagRef passes are not implemented on the 64-bit coefficient path");
-    launch_ht_decode_wide(d_dec.as<DecBlock>(), nb, max_block_w, cs_dev, d_coef.as<uint32_t>(), d_tables_dec.as<uint16_t>(), false,
-                          d_bstatus.as<uint32_t>(), stream);
-  } else
-    launch_ht_decode_serial(d_dec.as<DecBlock>(), nb, nfast, max_block_w, cs_dev, d_coef.as<uint32_t>(), d_scratch.as<uint32_t>(),
-                            d_tables_dec.as<uint16_t>(), dec_out, cleanup_only,
-                            d_bstatus.as<uint32_t>(), stream, &side);
-  last_launches += 1 + (nfast ? 1 : 0) + (nfast < nb ? 1 : 0);
+  enqueue_blocks(bf, hy, cs_dev, d_coef.as<uint32_t>(), stream, &side, last_launches);
   mark(3);
   if (nb) { launch_ctrl_copy(h_bstatus.p, d_bstatus.p, (size_t)nb * 4, stream); ++last_launches; }
   if (caller_image) enqueue_caller_image();
@@ -1594,6 +1635,146 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool call
   for (uint32_t b = 0; b < nb; ++b) if (bs[b] & 1u) ++failed_blocks;
   if (failed_blocks && !resilient) fail(0x000300A1, "Error decoding a codeblock.");
   return failed_blocks;
+}
+
+} // namespace ojb
+
+namespace ojb {
+
+//------------------------------------------------------------------------------------------
+// Transcoder (see ojb_codec.h)
+//------------------------------------------------------------------------------------------
+// The input's parse, what it refuses and the configuration it implies: the input's coding parameters, its main header
+// without TLM / PLM, its tile-part division and whether it had a TLM.  The encoder is configured again only when that
+// changed, and only after every check passed, so a refused input leaves the encoder as it was.
+void Encoder::transcode_parse(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type) {
+  if (!src) { src.reset(new Decoder()); src->parse_only = true; }
+  Decoder& D = *src;
+  if (on_device) D.read_headers_device(j2c, len, sample_type); else D.read_headers(j2c, len, sample_type);
+  if (D.params.uses_sop() || D.params.uses_eph())
+    fail(0x000B004C, "the codestream uses SOP or EPH markers (Scod bits 1-2), which a transcode does not write");
+  if (D.wide)
+    fail(0x000B0050, "a transcode needs the 32-bit coefficient path: this configuration codes 64-bit coefficients");
+  const uint8_t* d = D.j2c;
+  std::vector<uint8_t> hdr(d, d + 2);              // SOC
+  bool tlm = false;
+  for (size_t q = 2; q < D.first_sot; ) {
+    if (q + 4 > D.first_sot) fail(0x000B0051, "the codestream's main header is damaged");
+    const uint32_t m = ((uint32_t)d[q] << 8) | d[q + 1], L = ((uint32_t)d[q + 2] << 8) | d[q + 3];
+    if (q + 2 + L > D.first_sot) fail(0x000B0051, "the codestream's main header is damaged");
+    if (m == M_POC || m == M_PPM)
+      fail(0x000B004D, "the codestream has a %s segment, which changes where packet headers are or their order",
+           m == M_POC ? "POC" : "PPM");
+    if (m == M_TLM) tlm = true;
+    else if (m != M_PLM) hdr.insert(hdr.end(), d + q, d + q + 2 + L);
+    q += 2 + L;
+  }
+  try { D.parse_tiles(); }
+  catch (const Error& e) { fail(0x000B0051, "the codestream is truncated or damaged: %s", e.what()); }
+  if (D.tp_segments & 2u)
+    fail(0x000B004D, "a tile-part header has a PPT or POC segment, which changes where packet headers are or their order");
+  if (D.tp_segments & 1u)
+    fail(0x000B004E, "a tile-part header carries a marker segment other than PLT; a transcode writes none");
+  // the tile-part division: where the input's tile-parts start in each tile's packet sequence, against the four
+  // divisions the header plan writes (none, resolutions, components, both)
+  const uint32_t ntiles = (uint32_t)D.layout.tiles.size();
+  std::vector<PacketRef> seq; std::vector<uint32_t> tpf;
+  const uint32_t div0 = D.params.tilepart_div;
+  int div = -1;
+  for (uint32_t v = 0; v < 4 && div < 0; ++v) {
+    D.params.tilepart_div = v;
+    bool ok = true;
+    for (uint32_t t = 0; t < ntiles && ok; ++t) {
+      D.layout.packet_sequence(t, seq, tpf);
+      if (D.pkts_read[t] < seq.size()) { D.params.tilepart_div = div0; fail(0x000B0051, "the codestream is truncated: tile %u lacks packets", t); }
+      ok = tpf == D.tp_starts[t];
+    }
+    if (ok) div = (int)v;
+  }
+  D.params.tilepart_div = div0;
+  if (div < 0)
+    fail(0x000B004F, "the codestream's tile-parts follow none of the divisions a transcode writes (none, by resolution, by "
+         "component, by both)");
+  if (transcoding && hdr == main_header && params.tilepart_div == (uint32_t)div && params.need_tlm == tlm && img_type == sample_type)
+    return;
+  transcoding = false;                  // a failing setup leaves no half-configured transcoder
+  params = D.params;
+  params.tilepart_div = (uint32_t)div; params.need_tlm = tlm;
+  main_header.swap(hdr);
+  transcoding = true;
+  try { setup(sample_type); } catch (...) { transcoding = false; throw; }
+}
+
+void Encoder::transcode_headers(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type) {
+  transcoding = false;
+  transcode_parse(j2c, len, on_device, sample_type);
+}
+
+// the transform's place in the frame: the input to the device, [the source of a quality target: the input decoded as
+// the decoder would, synthesised into d_image], the coded words into d_coef and the frame's block array
+void Encoder::enqueue_transcode_front() {
+  Decoder& D = *src;
+  const uint32_t nb = (uint32_t)D.h_dec_proto.size();
+  if (xc_cs == D.d_cs.as<uint8_t>()) {
+    CK(cudaMemcpyAsync(D.d_cs.p, D.j2c, D.j2c_len, cudaMemcpyHostToDevice, stream));
+    CK(cudaMemsetAsync(D.d_cs.as<uint8_t>() + D.j2c_len, 0, 32, stream));
+  }
+  if (rq_on() && rq_planned) {
+    D.enqueue_blocks(xc_source, h_xdyn.as<DecDyn>(), xc_cs, d_rcoef.as<uint32_t>(), stream, &side, last_launches);
+    for (size_t li = rq_jobs.size(); li-- > 0; )
+      for (const JobGroup& g : rq_jobs[li]) {
+        if (g.stream)
+          launch_dwt_inv_stream(d_rq_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
+                                g.first, img_type, img_slot(false), false, d_rcoef.as<uint32_t>(), stream);
+        else
+          launch_dwt_inv(d_rq_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
+                         img_slot(false), d_rcoef.as<uint32_t>(), stream, false);
+        ++last_launches;
+      }
+  }
+  D.enqueue_blocks(xc_coded, D.h_dyn.as<DecDyn>(), xc_cs, d_coef.as<uint32_t>(), stream, &side, last_launches);
+  if (nb) { launch_ctrl_copy(D.h_bstatus.p, D.d_bstatus.p, (size_t)nb * 4, stream); ++last_launches; }
+  launch_transcode_blocks(d_blocks.as<EncBlock>(), D.d_dec.as<DecBlock>(), nb, d_xblocks.as<EncBlock>(), stream);
+  ++last_launches;
+}
+
+size_t Encoder::transcode(const uint8_t* j2c, size_t len, bool on_device, uint8_t* out, size_t out_cap, bool out_on_device) {
+  if (!transcoding)
+    fail(0x000B0052, "a transcode needs ojb_enc_transcode_headers first: this encoder is not configured from a codestream");
+  const auto t0 = std::chrono::steady_clock::now();
+  transcode_parse(j2c, len, on_device, img_type);
+  Decoder& D = *src;
+  const uint32_t nb = (uint32_t)D.h_dec_proto.size();
+  DecDyn* hy = D.h_dyn.as<DecDyn>();
+  xc_coded = D.frame_records(DEC_OUT_CODED, hy);
+  // what the block decoders and the encoder's slots rely on: every block's bytes inside the stream, and its lowest
+  // coded plane q_b at or above its band's least significant one (31 - K_max)
+  xc_two_pass = false;
+  for (uint32_t b = 0; b < nb; ++b) {
+    const DecDyn& y = hy[b];
+    if (y.num_passes == 0 || y.len1 == 0) continue;
+    if (y.data_off + y.len1 + y.len2 > len) fail(0x000B0051, "the codestream is truncated: code-block %u runs past its end", b);
+    const bool refined = y.num_passes > 1 && y.len2 != 0 && y.missing_msbs < 29;
+    if (y.missing_msbs >= 30 || (refined ? 29u : 30u) - y.missing_msbs < 31u - D.block_static[b].K_max)
+      fail(0x000B0051, "code-block %u of the codestream cannot be decoded: %u missing MSBs", b, (uint32_t)y.missing_msbs);
+    if (refined && y.num_passes == 2) xc_two_pass = true;
+  }
+  if (rq_on()) {
+    h_xdyn.reserve(std::max<size_t>(1, nb) * sizeof(DecDyn));
+    xc_source = D.frame_records(D.native_out(), h_xdyn.as<DecDyn>());
+  }
+  if (on_device) xc_cs = j2c;
+  else { D.d_cs.reserve(len + 64); xc_cs = D.d_cs.as<uint8_t>(); }
+  const float parse_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  phase = PHASE_TRANSCODE;
+  size_t n = 0;
+  try { n = encode(nullptr, nullptr, false, out, out_cap, out_on_device); } catch (...) { phase = PHASE_ALL; throw; }
+  phase = PHASE_ALL;
+  host_ms = parse_ms;
+  const uint32_t* bs = D.h_bstatus.as<uint32_t>();
+  for (uint32_t b = 0; b < nb; ++b)
+    if (bs[b] & 1u) fail(0x000B0051, "code-block %u of the codestream failed to decode", b);
+  return n;
 }
 
 } // namespace ojb

@@ -73,7 +73,7 @@ public:
   // skip_read >= skip_recon levels are not decoded (their bands read as zero)
   uint32_t skip_read = 0, skip_recon = 0;
   size_t img_bytes = 0;
-  void plan_image(uint32_t sample_type);
+  void plan_image(uint32_t sample_type, bool alloc = true);     // alloc = false: the planes' geometry only, no d_image
   // The image as the first-level DWT jobs reach it: one ImgComp per component in device memory.  Slot 0 describes
   // d_image (written by plan_image), slot 1 the caller's memory of a *_device call: the frame's own work copies it
   // from h_img, so a captured frame graph replays with whatever buffers the next call names.
@@ -126,11 +126,18 @@ public:
   bool no_fast_blocks = getenv("OJB_NO_FAST_BLOCKS") != nullptr;   // force the general block-coder kernels (tests, A/B)
 };
 
+class Decoder;
+// one frame's block decode (Decoder::frame_records): the output mode, blocks through the specialised kernel, whether
+// no block has refinement passes
+struct BlockFrame { uint32_t nfast = 0, dec_out = 0; bool cleanup_only = true; };
+
 class Encoder : public CodecBase {
 public:
   ~Encoder();
   // finalises parameters, builds geometry and device arenas, produces the main header
   void configure(const Params& p, uint32_t sample_type);
+  // configure's part after the main header: geometry, arenas, block tables, header plan (params and main_header set)
+  void setup(uint32_t sample_type);
   // encode one frame whose component planes are on the host (pinned or pageable; planes[c] points at sample (0,0) of
   // component c, stride in samples), already in d_image (planes == nullptr), or in the caller's device memory
   // (caller_image: described by use_caller_image)
@@ -138,7 +145,9 @@ public:
                 uint8_t* out, size_t out_cap, bool out_on_device);
   uint32_t status_flags = 0;
   // row regions (ojb_shard.cpp): the frame call split at the point where code-block bytes change hands
-  enum Phase : uint32_t { PHASE_ALL = 0, PHASE_FRONT = 1, PHASE_BACK = 2 };
+  // PHASE_TRANSCODE: the frame's coefficients come from an input codestream's code-blocks (transcode) instead of the
+  // forward DWT; everything after the transform runs as in PHASE_ALL
+  enum Phase : uint32_t { PHASE_ALL = 0, PHASE_FRONT = 1, PHASE_BACK = 2, PHASE_TRANSCODE = 3 };
   uint32_t phase = PHASE_ALL;
   // line-based front end (ojph::codestream::exchange): lines go to a pinned frame
   PinnedBuf h_frame;
@@ -210,6 +219,26 @@ public:
   void check_target_mse() const;
   void plan_quality();
   bool rq_on() const { return target_mse > 0; }
+  // Transcoding: the encoder configured from a codestream's headers and tile-parts (transcode_headers), and every
+  // frame re-coded from that codestream's code-blocks (transcode), single-layer and cleanup-only, to the encoder's
+  // target.  A parse-only decoder (no arena, image or synthesis jobs of its own) reads the input; its block decoders
+  // write the coded sign-magnitude words (DEC_OUT_CODED) into d_coef, whose band planes sit where the decoder's do
+  // (one Layout of one parameter set).  d_xblocks is the frame's block array: block b at p = q_b, the lowest plane the
+  // input codes it down to (31: left out), so candidate k = 0 re-codes exactly the input's bits; rate control and the
+  // block coder read it in place of d_blocks.  With a quality target the source is the input decoded as the decoder
+  // would, into d_rcoef and through rq_jobs into d_image, which exists only then.
+  std::unique_ptr<Decoder> src;
+  bool transcoding = false;
+  bool xc_two_pass = false;            // the frame has SigProp-without-MagRef blocks: k = 0 is not the source
+  DeviceBuf d_xblocks;
+  PinnedBuf h_xdyn;                    // the source decode's block records (the coded decode's sit in src->h_dyn)
+  const uint8_t* xc_cs = nullptr;      // the input on the device
+  BlockFrame xc_coded, xc_source;      // the frame's two block decodes (the source: with a quality target only)
+  void transcode_headers(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type);
+  size_t transcode(const uint8_t* j2c, size_t len, bool on_device, uint8_t* out, size_t out_cap, bool out_on_device);
+  void transcode_parse(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type);
+  void enqueue_transcode_front();
+  const EncBlock* frame_blocks() { return phase == PHASE_TRANSCODE ? d_xblocks.as<EncBlock>() : d_blocks.as<EncBlock>(); }
 };
 
 struct FrameInfo {
@@ -259,7 +288,24 @@ public:
   DeviceBuf d_cs, d_dec, d_proto, d_scratch, d_bstatus;
   PinnedBuf h_dyn, h_bstatus;
   bool any_rev_blocks = false, any_irv_blocks = false;
+  uint32_t native_out() const {
+    return (any_rev_blocks && any_irv_blocks) ? (uint32_t)DEC_OUT_PER_BLOCK : any_irv_blocks ? (uint32_t)DEC_OUT_FLOAT : (uint32_t)DEC_OUT_INT;
+  }
   void parse_tiles();
+  // what parse_tiles saw of the tile-parts: per tile, the packet each tile-part starts with; tile-part header segments
+  // (bit 0: other than PLT, bit 1: PPT or POC)
+  std::vector<std::vector<uint32_t>> tp_starts;
+  std::vector<uint32_t> pkts_read;     // per tile: packets parsed
+  uint32_t tp_segments = 0;
+  // the transcoder's parse (Encoder::transcode_headers): read_headers allocates no coefficient arena, image, synthesis
+  // jobs or refinement scratch (enqueue_blocks reserves the scratch when a frame has refinement passes)
+  bool parse_only = false;
+  size_t scratch_words = 0;
+  // the block records of the parsed frame into hy, for the output mode dec_out; the block decoders of those records
+  // into the arena coef on stream st (launches counted)
+  BlockFrame frame_records(uint32_t dec_out, DecDyn* hy);
+  void enqueue_blocks(const BlockFrame& f, const DecDyn* hy, const uint8_t* cs, uint32_t* coef, cudaStream_t st,
+                      const SideStream* sd, uint32_t& launches);
 };
 
 

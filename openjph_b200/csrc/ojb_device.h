@@ -148,7 +148,9 @@ enum : uint32_t {       // DecBlock output modes
   DEC_OUT_SIGNMAG = 0,  // raw sign-magnitude (kernel-level parity with ojph_decode_codeblock32)
   DEC_OUT_INT = 1,      // reversible: signed integers (tx_from_cb32 fused)
   DEC_OUT_FLOAT = 2,    // irreversible: float coefficient (tx_from_cb32 fused)
-  DEC_OUT_PER_BLOCK = 3 // INT or FLOAT by the block's flags (components may differ: COC)
+  DEC_OUT_PER_BLOCK = 3,// INT or FLOAT by the block's flags (components may differ: COC)
+  DEC_OUT_CODED = 4     // transcoding: the sign-magnitude word with every bit below the lowest coded plane cleared (no
+                        // bin centre): the encoder's band-plane format, which the block encoder re-codes bit for bit
 };
 
 // ---- DWT --------------------------------------------------------------------------------

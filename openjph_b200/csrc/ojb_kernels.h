@@ -31,6 +31,9 @@ void launch_ht_decode_serial(const DecBlock* blocks, uint32_t nblocks, uint32_t 
 // per-frame block records: blocks[b] = proto[b] with the frame's fields (dyn) applied.
 // dyn may be mapped pinned host memory (read by the SMs, like launch_ctrl_copy)
 void launch_dec_merge(DecBlock* blocks, const DecBlock* proto, const DecDyn* dyn, uint32_t nblocks, cudaStream_t st);
+// transcoding: out[b] = geom[b] (the encoder's static block array) with p = q_b, the lowest plane the merged decoder
+// record dec[b] codes (31: the block is left out)
+void launch_transcode_blocks(const EncBlock* geom, const DecBlock* dec, uint32_t nblocks, EncBlock* out, cudaStream_t st);
 
 // 64-bit samples (precision beyond 32 bits): cleanup pass only, output int64 (or the raw sign-magnitude words)
 void launch_ht_decode_wide(const DecBlock* blocks, uint32_t nblocks, uint32_t max_width, const uint8_t* codestream,
@@ -94,8 +97,9 @@ double colour_weight(bool ict, uint32_t c);
 // (the decoder's inverse DWT launches then synthesise it); the round's exact squared error and the bracket update;
 // the final selection at t_pass
 void launch_rq_init(const RcTables& t, uint64_t limit, uint32_t ncomp, bool lossless0, cudaStream_t st);
-void launch_rq_select(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res, const uint32_t* coef,
-                      uint32_t* recon, const RcTables& t, cudaStream_t st);
+// (geom: the static block array, whose p = 31 - K_max is the decoder's integer shift; blocks: where each block starts)
+void launch_rq_select(const EncBlock* geom, const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res,
+                      const uint32_t* coef, uint32_t* recon, const RcTables& t, cudaStream_t st);
 void launch_rq_measure(const ImgComp* decoded, const ImgComp* source, const RqImage& im, const RcTables& t, cudaStream_t st);
 void launch_rq_final(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res, const RcTables& t, cudaStream_t st);
 // block pieces computed on the device from per-block results + destination offsets

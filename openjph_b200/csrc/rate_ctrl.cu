@@ -308,15 +308,17 @@ __global__ void rq_init_kernel(RcTables t, unsigned long long limit, uint32_t nc
 }
 
 // one warp per block: block b coded at p + k decodes to sign | ((m >> k) << (p + k)) | 2^(p + k - 1) for every
-// sample whose m >> k is not 0, and to 0 for the others; to_output turns that into the value the decoder stores
+// sample whose m >> k is not 0, and to 0 for the others; to_output turns that into the value the decoder stores (its
+// integer shift is 31 - K_max, the p of the static block array geom: a transcoded block starts at or below K_max)
 __global__ void __launch_bounds__(128)
-rq_recon_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks, const uint32_t* __restrict__ coef, uint32_t* __restrict__ out, RcTables t)
+rq_recon_kernel(const EncBlock* __restrict__ geom, const EncBlock* __restrict__ blocks, uint32_t nblocks, const uint32_t* __restrict__ coef,
+                uint32_t* __restrict__ out, RcTables t)
 {
   const uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
   if (b >= nblocks || t.q->done) return;
   const EncBlock blk = blocks[b];
   const uint32_t p = blk.p, k = t.chosen[b], pk = p + k;
-  const uint32_t mode = t.irv[b] ? (uint32_t)DEC_OUT_FLOAT : (uint32_t)DEC_OUT_INT;
+  const uint32_t mode = t.irv[b] ? (uint32_t)DEC_OUT_FLOAT : (uint32_t)DEC_OUT_INT, shift = geom[b].p;
   const float delta = t.delta[b];
   const uint32_t* src = coef + blk.src_off;
   uint32_t* dst = out + blk.src_off;
@@ -324,7 +326,7 @@ rq_recon_kernel(const EncBlock* __restrict__ blocks, uint32_t nblocks, const uin
     for (uint32_t x = lane; x < blk.w; x += 32) {
       const uint32_t w = src[(size_t)y * blk.stride + x];
       const uint32_t m = ((w & 0x7FFFFFFFu) >> p) >> k;
-      dst[(size_t)y * blk.stride + x] = m ? to_output((w & 0x80000000u) | (m << pk) | (1u << (pk - 1)), mode, p, delta) : 0u;
+      dst[(size_t)y * blk.stride + x] = m ? to_output((w & 0x80000000u) | (m << pk) | (1u << (pk - 1)), mode, shift, delta) : 0u;
     }
 }
 
@@ -423,11 +425,11 @@ void launch_rc_check(const RcTables& t, const uint64_t* total, uint64_t target, 
 void launch_rq_init(const RcTables& t, uint64_t limit, uint32_t ncomp, bool lossless0, cudaStream_t st) {
   OJB_LAUNCH(rq_init_kernel, dim3(1), dim3(1), 0, st, t, (unsigned long long)limit, ncomp, lossless0 ? 1u : 0u);
 }
-void launch_rq_select(const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res, const uint32_t* coef,
-                      uint32_t* recon, const RcTables& t, cudaStream_t st) {
+void launch_rq_select(const EncBlock* geom, const EncBlock* blocks, uint32_t nblocks, EncBlock* work, EncResult* res,
+                      const uint32_t* coef, uint32_t* recon, const RcTables& t, cudaStream_t st) {
   OJB_LAUNCH(rc_select_kernel<true>, dim3(1), dim3(RS_THREADS), 0, st, nblocks, t);
   OJB_LAUNCH(rc_apply_kernel<1>, dim3((nblocks + 127) / 128), dim3(128), 0, st, blocks, nblocks, work, res, t);
-  OJB_LAUNCH(rq_recon_kernel, dim3((nblocks + 3) / 4), dim3(128), 0, st, blocks, nblocks, coef, recon, t);
+  OJB_LAUNCH(rq_recon_kernel, dim3((nblocks + 3) / 4), dim3(128), 0, st, geom, blocks, nblocks, coef, recon, t);
 }
 void launch_rq_measure(const ImgComp* decoded, const ImgComp* source, const RqImage& im, const RcTables& t, cudaStream_t st) {
   uint32_t rows = 1;
