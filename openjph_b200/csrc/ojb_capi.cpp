@@ -1,7 +1,6 @@
 // ojb_capi.cpp -- the extern "C" surface declared in include/ojph_b200.h.
 #include "../../include/ojph_b200.h"
 #include "ojb_codec.h"
-#include "ht_tables.h"
 #include <cstring>
 #include <new>
 #include <algorithm>
@@ -226,7 +225,7 @@ static uint64_t raster_geometry(CodecBase& cb, uint32_t layout, uint32_t& es, Ra
   const uint32_t nc = P.num_comps();
   if (layout > 3) fail(0x000B0030, "unknown raster layout");
   if (cb.img_type == ST_I32) fail(0x000B0031, "file payloads need the 8-bit or 16-bit sample container");
-  es = cb.img_type == ST_U8 ? 1u : 2u;
+  es = esize_of(cb.img_type);
   uint64_t total = 0;
   for (uint32_t c = 0; c < nc; ++c) {
     if ((P.comps[c].bit_depth > 8) != (es == 2))
@@ -321,24 +320,10 @@ int ojb_dec_decode_raster(ojb_decoder* d, uint32_t layout, void* payload, uint64
 // device-side accessors
 namespace ojb {
 static void* img_plane(CodecBase& cb, uint32_t c) { return cb.d_image.as<uint8_t>() + cb.img_off[c]; }
-static void upload_frame(Encoder& E, const void* const* planes, const uint32_t* strides) {
-  uint32_t es = E.img_type == ST_U8 ? 1u : (E.img_type == ST_U16 ? 2u : 4u);
-  for (uint32_t c = 0; c < E.params.num_comps(); ++c) {
-    uint8_t* d = E.d_image.as<uint8_t>() + E.img_off[c];
-    uint32_t st = strides ? strides[c] : E.img_w[c];
-    if (st == E.img_w[c])
-      cuda_check(cudaMemcpyAsync(d, planes[c], (size_t)E.img_w[c] * E.img_h[c] * es, cudaMemcpyHostToDevice, E.stream), "upload");
-    else
-      for (uint32_t y = 0; y < E.img_h[c]; ++y)
-        cuda_check(cudaMemcpyAsync(d + (size_t)y * E.img_w[c] * es, (const uint8_t*)planes[c] + (size_t)y * st * es,
-                                   (size_t)E.img_w[c] * es, cudaMemcpyHostToDevice, E.stream), "upload");
-  }
-  cuda_check(cudaStreamSynchronize(E.stream), "upload sync");
-}
 // the caller's image (ojb_device_image) checked against the component sizes of ojb_frame_info
 static void caller_image(const CodecBase& cb, const ojb_device_image* in, std::vector<ImgComp>& comps) {
   const uint32_t nc = cb.params.num_comps();
-  const uint64_t es = cb.img_type == ST_U8 ? 1u : (cb.img_type == ST_U16 ? 2u : 4u);
+  const uint64_t es = esize_of(cb.img_type);
   comps.assign(nc, ImgComp());
   for (uint32_t c = 0; c < nc; ++c) {
     const uint64_t base = in ? (uint64_t)(uintptr_t)in->base[c] : 0, pitch = in ? in->row_pitch[c] : 0;
@@ -382,7 +367,8 @@ int ojb_enc_upload_frame(ojb_encoder* e, const void* const* planes, const uint32
   return guarded_on(e->device, [&] {
     if (!e->configured) fail(0x000B0013, "encoder is not configured");
     if (e->enc.transcoding) fail(0x000B0053, "this encoder was configured from a codestream: it transcodes, it has no image");
-    upload_frame(e->enc, planes, strides);
+    e->enc.upload_planes(planes, strides);
+    cuda_check(cudaStreamSynchronize(e->enc.stream), "upload sync");
   });
 }
 int ojb_enc_encode_device(ojb_encoder* e, const ojb_device_image* in, void* cuda_stream,
@@ -703,15 +689,10 @@ int ojb_dec_read_band(ojb_decoder* d, uint32_t tile, uint32_t comp, uint32_t res
 int ojb_encode_blocks(const uint32_t* samples, uint64_t n_words, ojb_block_desc* desc, uint32_t n,
                       uint8_t* bytes, uint64_t bytes_cap, uint64_t* bytes_used) {
   return guarded([&] {
-    const HtTables& t = ht_tables();
-    std::vector<uint16_t> tb(2 * 2048 + 36, 0);
-    memcpy(tb.data(), t.enc_vlc, sizeof(t.enc_vlc));
-    memcpy(tb.data() + 2 * 2048, t.enc_uvlc, sizeof(t.enc_uvlc));
     DeviceBuf d_s, d_b, d_r, d_t, d_sl, d_st;
     d_s.reserve((n_words + 64) * 4);
     cuda_check(cudaMemcpy(d_s.p, samples, n_words * 4, cudaMemcpyHostToDevice), "samples");
-    d_t.reserve(tb.size() * 2);
-    cuda_check(cudaMemcpy(d_t.p, tb.data(), tb.size() * 2, cudaMemcpyHostToDevice), "tables");
+    upload_ht_tables(true, d_t);
     std::vector<EncBlock> eb(n);
     uint64_t slot = 0;
     uint32_t nfast = 0;
@@ -720,12 +701,8 @@ int ojb_encode_blocks(const uint32_t* samples, uint64_t n_words, ojb_block_desc*
         fail(0x000B0021, "unsupported code-block geometry");
       eb[i].src_off = desc[i].sample_off; eb[i].stride = desc[i].stride; eb[i].w = (uint16_t)desc[i].w; eb[i].h = (uint16_t)desc[i].h;
       eb[i].p = (uint16_t)(30u - desc[i].missing_msbs);
-      uint64_t kmax = desc[i].missing_msbs + 1;
-      uint64_t ms = ((uint64_t)desc[i].w * desc[i].h * (kmax + 1) + 7) / 8; ms += ms / 15 + 8;
-      uint64_t nq = (uint64_t)((desc[i].w + 1) / 2) * ((desc[i].h + 1) / 2);
-      uint64_t vl = ((nq + 1) / 2 * 30 + 12 + 7) / 8; vl += vl / 7 + 8;
-      uint64_t cap = (ms + vl + 192 + 160 + 15) & ~(uint64_t)15;
-      eb[i].slot_off = slot; eb[i].slot_cap = (uint32_t)cap; slot += cap;
+      eb[i].slot_off = slot; eb[i].slot_cap = enc_slot_cap(desc[i].w, desc[i].h, desc[i].missing_msbs + 1, false);
+      slot += eb[i].slot_cap;
       if (!getenv("OJB_NO_FAST_BLOCKS") && enc_block_is_fast(eb[i])) { eb[i].flags |= ENC_FLAG_FAST; ++nfast; }
     }
     d_b.reserve(n * sizeof(EncBlock)); d_r.reserve(n * sizeof(EncResult)); d_sl.reserve(slot + 64); d_st.reserve(64);
@@ -761,17 +738,11 @@ int ojb_encode_blocks(const uint32_t* samples, uint64_t n_words, ojb_block_desc*
 int ojb_decode_blocks(const uint8_t* bytes, uint64_t n_bytes, ojb_block_desc* desc, uint32_t n,
                       uint32_t* samples, uint64_t n_words) {
   return guarded([&] {
-    const HtTables& t = ht_tables();
-    std::vector<uint16_t> tb(1024 * 2 + 320 + 256);
-    memcpy(tb.data(), t.dec_vlc, sizeof(t.dec_vlc));
-    memcpy(tb.data() + 2048, t.dec_uvlc0, sizeof(t.dec_uvlc0));
-    memcpy(tb.data() + 2048 + 320, t.dec_uvlc1, sizeof(t.dec_uvlc1));
     DeviceBuf d_cs, d_b, d_t, d_o, d_sc, d_st;
     d_cs.reserve(n_bytes + 64);
     cuda_check(cudaMemset(d_cs.p, 0, d_cs.cap), "cs");
     cuda_check(cudaMemcpy(d_cs.p, bytes, n_bytes, cudaMemcpyHostToDevice), "cs");
-    d_t.reserve(tb.size() * 2);
-    cuda_check(cudaMemcpy(d_t.p, tb.data(), tb.size() * 2, cudaMemcpyHostToDevice), "tables");
+    upload_ht_tables(false, d_t);
     std::vector<DecBlock> db(n);
     size_t scratch = 0;
     uint32_t nfast = 0;

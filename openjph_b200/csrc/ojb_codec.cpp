@@ -63,22 +63,25 @@ CodecBase::~CodecBase() {
   if (stream) cudaStreamDestroy(stream);
 }
 
-void CodecBase::upload_tables() {
+void upload_ht_tables(bool enc, DeviceBuf& dev) {
   const HtTables& t = ht_tables();
-  std::vector<uint16_t> e(2 * 2048 + 36, 0);
-  memcpy(e.data(), t.enc_vlc, sizeof(t.enc_vlc));
-  memcpy(e.data() + 2 * 2048, t.enc_uvlc, sizeof(t.enc_uvlc));
-  d_tables_enc.reserve(e.size() * 2);
-  CK(cudaMemcpy(d_tables_enc.p, e.data(), e.size() * 2, cudaMemcpyHostToDevice));
-  std::vector<uint16_t> d(1024 * 2 + 320 + 256);
-  memcpy(d.data(), t.dec_vlc, sizeof(t.dec_vlc));
-  memcpy(d.data() + 2048, t.dec_uvlc0, sizeof(t.dec_uvlc0));
-  memcpy(d.data() + 2048 + 320, t.dec_uvlc1, sizeof(t.dec_uvlc1));
-  d_tables_dec.reserve(d.size() * 2);
-  CK(cudaMemcpy(d_tables_dec.p, d.data(), d.size() * 2, cudaMemcpyHostToDevice));
+  std::vector<uint16_t> w(enc ? 2 * 2048 + 36 : 1024 * 2 + 320 + 256, 0);
+  if (enc) {
+    memcpy(w.data(), t.enc_vlc, sizeof(t.enc_vlc));
+    memcpy(w.data() + 2 * 2048, t.enc_uvlc, sizeof(t.enc_uvlc));
+  } else {
+    memcpy(w.data(), t.dec_vlc, sizeof(t.dec_vlc));
+    memcpy(w.data() + 2048, t.dec_uvlc0, sizeof(t.dec_uvlc0));
+    memcpy(w.data() + 2048 + 320, t.dec_uvlc1, sizeof(t.dec_uvlc1));
+  }
+  dev.reserve(w.size() * 2);
+  CK(cudaMemcpy(dev.p, w.data(), w.size() * 2, cudaMemcpyHostToDevice));
 }
 
-static inline uint32_t esize_of(uint32_t st) { return st == ST_U8 ? 1u : (st == ST_U16 ? 2u : 4u); }
+void CodecBase::upload_tables() {
+  upload_ht_tables(true, d_tables_enc);
+  upload_ht_tables(false, d_tables_dec);
+}
 
 void CodecBase::plan_image(uint32_t sample_type, bool alloc) {
   img_type = sample_type;
@@ -413,6 +416,24 @@ void CodecBase::build_dwt_jobs(bool forward, std::vector<std::vector<JobGroup>>&
     CK(cudaMemcpy(d_jobs.as<DwtJob>() + g.dev_off, g.jobs.data(), g.jobs.size() * sizeof(DwtJob), cudaMemcpyHostToDevice));
 }
 
+void CodecBase::enqueue_dwt(bool forward, const std::vector<std::vector<JobGroup>>& groups, DeviceBuf& dev,
+                            const ImgComp* img, bool interleaved, uint32_t* coef) {
+  for (size_t i = 0; i < groups.size(); ++i)
+    for (const JobGroup& g : groups[forward ? i : groups.size() - 1 - i]) {
+      const DwtJob* j = dev.as<DwtJob>() + g.dev_off;
+      const uint32_t n = (uint32_t)g.jobs.size();
+      if (forward && g.stream)
+        launch_dwt_fwd_stream(j, n, g.ctas, g.reversible, g.ncomp, g.first, img_type, img, interleaved, coef, stream);
+      else if (forward)
+        launch_dwt_fwd(j, n, g.ctas, g.reversible, g.ncomp, img, coef, stream, wide);
+      else if (g.stream)
+        launch_dwt_inv_stream(j, n, g.ctas, g.reversible, g.ncomp, g.first, img_type, img, interleaved, coef, stream);
+      else
+        launch_dwt_inv(j, n, g.ctas, g.reversible, g.ncomp, img, coef, stream, wide);
+      ++last_launches;
+    }
+}
+
 // widest nominal code-block; blocks wider than 64 samples go through the thread-per-block kernels
 // (the warp-per-block kernels keep one quad column per lane)
 static uint32_t widest_block(const Layout& L) {
@@ -428,6 +449,15 @@ static uint32_t widest_block(const Layout& L) {
 //------------------------------------------------------------------------------------------
 // Encoder
 //------------------------------------------------------------------------------------------
+uint32_t enc_slot_cap(uint32_t w, uint32_t h, uint32_t K_max, bool wide) {
+  // worst case: (K_max+1) MagSgn bits / sample (+1/15 stuffing), 30 VLC bits / quad pair
+  // (+1/7), 192 MEL bytes, working margin of the kernel
+  uint64_t ms = ((uint64_t)w * h * (K_max + 1) + 7) / 8; ms += ms / 15 + 8;
+  uint64_t nq = (uint64_t)((w + 1) / 2) * ((h + 1) / 2);
+  uint64_t vl = ((nq + 1) / 2 * (wide ? 38 : 30) + 12 + 7) / 8; vl += vl / 7 + 8;      // (+ two 4-bit U-VLC extensions per pair)
+  return (uint32_t)((ms + vl + 192 + 160 + 15) & ~(uint64_t)15);
+}
+
 void Encoder::configure(const Params& p, uint32_t sample_type) {
   params = p;
   params.finalize_for_encode();
@@ -465,15 +495,8 @@ void Encoder::setup(uint32_t sample_type) {
               e.stride = bg.plane_stride; e.w = (uint16_t)r.w; e.h = (uint16_t)r.h;
               e.p = (uint16_t)((wide ? 63u : 31u) - bg.K_max);
               e.flags = (tc.res.size() == 1 && params.reversible(tc.comp)) ? (uint16_t)ENC_CHECK_NEGZERO : (uint16_t)0;
-              // worst case: (K_max+1) MagSgn bits / sample (+1/15 stuffing), 30 VLC bits / quad pair
-              // (+1/7), 192 MEL bytes, working margin of the kernel
-              uint64_t ms = ((uint64_t)r.w * r.h * (bg.K_max + 1) + 7) / 8; ms += ms / 15 + 8;
-              uint64_t nq = (uint64_t)((r.w + 1) / 2) * ((r.h + 1) / 2);
-              uint64_t vl = ((nq + 1) / 2 * (wide ? 38 : 30) + 12 + 7) / 8; vl += vl / 7 + 8;      // (+ two 4-bit U-VLC extensions per pair)
-              uint64_t cap = ms + vl + 192 + 160;
-              cap = (cap + 15) & ~(uint64_t)15;
-              e.slot_off = slot; e.slot_cap = (uint32_t)cap;
-              slot += cap;
+              e.slot_off = slot; e.slot_cap = enc_slot_cap(r.w, r.h, bg.K_max, wide);
+              slot += e.slot_cap;
               if (!tile_wanted(t.idx)) { e.w = e.h = 0; }                  // another rank's tile: nothing to code
               if (region.on() && !region_blocks[bg.block_base + by * bg.nbw + bx]) { e.w = e.h = 0; }   // another rank's rows
               if (!no_fast_blocks && !wide && enc_block_is_fast(e)) { e.flags |= ENC_FLAG_FAST; ++num_fast_blocks; }
@@ -630,15 +653,20 @@ uint64_t Encoder::min_size_of_geometry() const {
 
 void Encoder::set_target(uint64_t bytes) {
   if (bytes && rq_on()) fail(0x000B0049, "a target size and a target quality cannot be combined on one encoder");
-  if (bytes && wide)
+  if (bytes) check_target_size(bytes);
+  target_bytes = bytes;
+}
+
+// what a size target needs of the configuration and of the geometry (a reconfigure may raise min_bytes past it)
+void Encoder::check_target_size(uint64_t bytes) const {
+  if (wide)
     fail(0x000B0039, "a target size needs the 32-bit coefficient path: this configuration codes 64-bit coefficients");
-  if (bytes && !rc_sizing)
+  if (!rc_sizing)
     fail(0x000B0039, "a target size needs every tile-part to hold a packet: the device header plan that sizes each "
          "selection cannot describe an empty tile-part");
-  if (bytes && bytes < min_bytes)
+  if (bytes < min_bytes)
     fail(0x000B0038, "target of %llu bytes is below the smallest codestream of this geometry (%llu bytes)",
          (unsigned long long)bytes, (unsigned long long)min_bytes);
-  target_bytes = bytes;
 }
 
 // what a quality target needs of the configuration: the size target's conditions (the selection and the final layout
@@ -787,270 +815,276 @@ int32_t* Encoder::exchange(const int32_t* line_written, uint32_t& next_comp) {
 size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool caller_image,
                        uint8_t* out, size_t out_cap, bool out_on_device)
 {
-  const Params& P = params;
-  uint32_t nc = P.num_comps(), es = esize_of(img_type);
-  if (transcoding && phase != PHASE_TRANSCODE)
+  if (transcoding)
     fail(0x000B0053, "this encoder was configured from a codestream (ojb_enc_transcode_headers): it transcodes, it has no image");
+  Frame f = begin_frame(Frame::DWT, true, caller_image, planes, strides);
+  f.graph = planes == nullptr && out_on_device;
+  return device_headers ? finish_device(f, out, out_cap, out_on_device) : finish_host(f, out, out_cap, out_on_device);
+}
+
+void Encoder::encode_front() {
+  const Frame f = begin_frame(Frame::DWT, false);
+  enqueue_front(f);
+  launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches;
+  mark(4);
+  CK(cudaStreamSynchronize(stream));
+  CK(cudaGetLastError());
+  collect(5);
+  check_coder_status();
+}
+
+size_t Encoder::encode_back(uint8_t* out, size_t out_cap) {
+  const Frame f = begin_frame(Frame::CODED, false);
+  return device_headers ? finish_device(f, out, out_cap, true) : finish_host(f, out, out_cap, true);
+}
+
+// stage marks 0 and 1 around the planes' upload; with a target (targets: a whole frame), its conditions and buffers
+Encoder::Frame Encoder::begin_frame(Frame::Front front, bool targets, bool caller_image, const void* const* planes,
+                                    const uint32_t* strides) {
   last_launches = 0;
   mark(0);
-  // 1. image planes -> device
-  if (planes) {
-    for (uint32_t c = 0; c < nc; ++c) {
-      uint8_t* d = d_image.as<uint8_t>() + img_off[c];
-      uint32_t st = strides ? strides[c] : img_w[c];
-      if (st == img_w[c])
-        CK(cudaMemcpyAsync(d, planes[c], (size_t)img_w[c] * img_h[c] * es, cudaMemcpyHostToDevice, stream));
-      else
-        for (uint32_t y = 0; y < img_h[c]; ++y)
-          CK(cudaMemcpyAsync(d + (size_t)y * img_w[c] * es, (const uint8_t*)planes[c] + (size_t)y * st * es,
-                             (size_t)img_w[c] * es, cudaMemcpyHostToDevice, stream));
-    }
-  }
+  if (planes) upload_planes(planes, strides);
   mark(1);
-  uint32_t nb = (uint32_t)h_blocks.size();
-  const bool whole = phase == PHASE_ALL || phase == PHASE_TRANSCODE;
-  const bool rq_frame = rq_on() && whole && nb > 0;
-  const bool rc_frame = (rc_on() && whole && nb > 0) || rq_frame;
-  if (rq_frame) {
+  Frame f;
+  f.front = front; f.caller_image = caller_image;
+  f.nb = (uint32_t)h_blocks.size();
+  f.rq = targets && rq_on() && f.nb > 0;
+  f.rc = (targets && rc_on() && f.nb > 0) || f.rq;
+  if (f.rq) {
     check_target_mse();
     if (rc_kc == 0) plan_rate_control();
     if (!rq_planned) plan_quality();
     rq_limit = sse_limit(target_mse, rq_samples);
     rq_valid = false;
-  } else if (rc_frame) {
-    if (wide) fail(0x000B0039, "a target size needs the 32-bit coefficient path: this configuration codes 64-bit coefficients");
-    if (target_bytes < min_bytes)
-      fail(0x000B0038, "target of %llu bytes is below the smallest codestream of this geometry (%llu bytes)",
-           (unsigned long long)target_bytes, (unsigned long long)min_bytes);
-    if (!rc_sizing)
-      fail(0x000B0039, "a target size needs every tile-part to hold a packet: the device header plan that sizes each "
-           "selection cannot describe an empty tile-part");
+  } else if (f.rc) {
+    check_target_size(target_bytes);
     if (rc_kc == 0) plan_rate_control();
   }
-  // rate control: the candidates and the rounds of the selection (rate_ctrl.cu); each round sizes its selection with the
-  // packet header kernels, so the block coder's final pass and the headers see the chosen planes in d_work
-  EncBlock* const work = d_work.as<EncBlock>();
-  const EncBlock* const blocks = frame_blocks();          // where each block starts (a transcode: at the input's plane)
-  const EncBlock* const code_blocks = rc_frame ? work : blocks;
-  auto rc_size = [&](bool first) {
-    launch_packet_header_total(hplan, work, d_results.as<EncResult>(), 30u, fixed_blob.size(), true, stream);
-    launch_rc_check(rc, hplan.total, target_bytes, min_bytes, first, stream);
-    last_launches += packet_header_total_launches(hplan) + 1;
-  };
-  auto rc_state_out = [&] {
-    launch_ctrl_copy(h_rc.p, rc.state, sizeof(RcState), stream);
-    launch_ctrl_copy(h_rc.as<uint8_t>() + 64, rc.chosen, nb, stream);
-    last_launches += 2;
-  };
-  // a round of the quality target: select, reconstruct as the decoder would, synthesise, measure (rate_ctrl.cu)
-  auto rq_round = [&] {
-    launch_rq_select(d_blocks.as<EncBlock>(), blocks, nb, work, d_results.as<EncResult>(), d_coef.as<uint32_t>(), d_rcoef.as<uint32_t>(), rc, stream);
-    last_launches += 3;
-    for (size_t li = rq_jobs.size(); li-- > 0; )
-      for (const JobGroup& g : rq_jobs[li]) {
-        if (g.stream)
-          launch_dwt_inv_stream(d_rq_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                                g.first, img_type, scratch_slot(), false, d_rcoef.as<uint32_t>(), stream);
-        else
-          launch_dwt_inv(d_rq_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                         scratch_slot(), d_rcoef.as<uint32_t>(), stream, false);
-        ++last_launches;
-      }
-    launch_rq_measure(scratch_slot(), img_slot(caller_image), rq_image, rc, stream);
-    last_launches += 2;
-  };
-  auto rq_final = [&] {
-    launch_rq_final(blocks, nb, work, d_results.as<EncResult>(), rc, stream);
-    launch_ctrl_copy(h_rq.p, rc.q, sizeof(RqState), stream);
-    launch_ctrl_copy(h_rc.as<uint8_t>() + 64, rc.chosen, nb, stream);
-    last_launches += 3;
-  };
-  auto enqueue_rc = [&] {
-    CK(cudaMemsetAsync(rc.state, 0, sizeof(RcState), stream));
-    launch_rc_prepare(blocks, nb, d_coef.as<uint32_t>(), rc, stream);
-    mark(8);
-    launch_ht_encode_lengths(blocks, nb, rc.kc, rc.ncand, max_block_w, d_coef.as<uint32_t>(), rc.cand,
-                             d_tables_enc.as<uint16_t>(), stream);
-    mark(9);
-    launch_rc_hull(blocks, nb, work, d_results.as<EncResult>(), rc, stream);
-    last_launches += 4;
-    if (rq_frame) {
-      CK(cudaMemsetAsync(rc.q, 0, sizeof(RqState), stream));
-      launch_rq_init(rc, rq_limit, P.num_comps(), rq_lossless0 && !(phase == PHASE_TRANSCODE && xc_two_pass), stream);
-      ++last_launches;
-      for (int r = 0; r < RQ_GRAPH_ROUNDS; ++r) rq_round();
-      rq_final();
-      mark(10);
-      return;
-    }
-    rc_size(true);
-    for (int r = 0; r < RC_ROUNDS; ++r) {
-      launch_rc_round(blocks, nb, work, d_results.as<EncResult>(), rc, stream);
-      last_launches += 2;
-      rc_size(false);
-    }
-    rc_state_out();
-    mark(10);
-  };
-  // after the frame's rounds: the rare selection that still does not fit goes on eagerly; true = it changed
-  auto rc_settle = [&]() -> bool {
-    if (rq_frame) {
-      if (h_rq.as<RqState>()->done) return false;
-      CK(cudaEventRecord(rq_ev[0], stream));
-      // the bracket closes within RQ_BODY_ROUNDS + 34 rounds (rq_update_kernel); one synchronisation per round
-      while (!h_rq.as<RqState>()->done) {
-        rq_round();
-        launch_ctrl_copy(h_rq.p, rc.q, sizeof(RqState), stream); ++last_launches;
-        CK(cudaStreamSynchronize(stream));
-      }
-      rq_final();
-      CK(cudaEventRecord(rq_ev[1], stream));
-      return true;
-    }
-    if (!rc_frame || h_rc.as<RcState>()->done) return false;
-    for (int i = 0; !h_rc.as<RcState>()->done; ++i) {
-      // every round over the target strictly lowers the selected body (rc_check_kernel), so there are at most as many
-      // rounds as distinct selections: one more hull segment per block and round at the very worst
-      if ((uint64_t)i > (uint64_t)nb * rc.kc + 2)
-        fail(0x000B003A, "rate control did not settle on a selection that fits the target (internal error)");
-      launch_rc_round(blocks, nb, work, d_results.as<EncResult>(), rc, stream);
-      last_launches += 2;
-      rc_size(false);
-      rc_state_out();
-      CK(cudaStreamSynchronize(stream));
-    }
-    return true;
-  };
-  const bool thread_per_block = (serial_block_encoder() && !few_blocks_warp) || max_block_w > 64 || wide;
-  auto enqueue_code = [&] {
-    if (thread_per_block)
-      launch_ht_encode_serial(code_blocks, nb, num_fast_blocks, max_block_w, d_coef.as<uint32_t>(), d_slots.as<uint8_t>(),
-                              d_results.as<EncResult>(), d_tables_enc.as<uint16_t>(), d_status.as<uint32_t>(), stream, wide, &side);
+  f.work = d_work.as<EncBlock>();
+  f.blocks = front == Frame::TRANSCODE ? d_xblocks.as<EncBlock>() : d_blocks.as<EncBlock>();
+  f.code_blocks = f.rc ? f.work : f.blocks;
+  return f;
+}
+
+void Encoder::upload_planes(const void* const* planes, const uint32_t* strides) {
+  const uint32_t es = esize_of(img_type);
+  for (uint32_t c = 0; c < params.num_comps(); ++c) {
+    uint8_t* d = d_image.as<uint8_t>() + img_off[c];
+    const uint32_t st = strides ? strides[c] : img_w[c];
+    if (st == img_w[c])
+      cuda_check(cudaMemcpyAsync(d, planes[c], (size_t)img_w[c] * img_h[c] * es, cudaMemcpyHostToDevice, stream), "upload");
     else
-      launch_ht_encode(code_blocks, nb, d_coef.as<uint32_t>(), d_slots.as<uint8_t>(),
-                       d_results.as<EncResult>(), d_tables_enc.as<uint16_t>(), d_status.as<uint32_t>(), stream);
-    last_launches += thread_per_block ? (num_fast_blocks ? 1 : 0) + (num_fast_blocks < nb ? 1 : 0) : 1;
-  };
-  // 2. transform + block coding (row regions, ojb_shard.cpp: PHASE_FRONT stops after it -- lengths and bytes of this
-  // rank's blocks then travel to the writer --, PHASE_BACK on the writer starts behind it)
-  auto enqueue_front = [&] {
+      for (uint32_t y = 0; y < img_h[c]; ++y)
+        cuda_check(cudaMemcpyAsync(d + (size_t)y * img_w[c] * es, (const uint8_t*)planes[c] + (size_t)y * st * es,
+                                   (size_t)img_w[c] * es, cudaMemcpyHostToDevice, stream), "upload");
+  }
+}
+
+// the transform (forward DWT or a transcode's block decoders), a target's selection and the block coding
+void Encoder::enqueue_front(const Frame& f) {
   CK(cudaMemsetAsync(d_status.p, 0, 16, stream));
-  if (caller_image) enqueue_caller_image();
-  if (phase == PHASE_TRANSCODE) enqueue_transcode_front();
-  else if (phase != PHASE_BACK)
-  for (size_t li = 0; li < jobs.size(); ++li)
-    for (const JobGroup& g : jobs[li]) {
-      if (g.stream)
-        launch_dwt_fwd_stream(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                              g.first, img_type, img_slot(caller_image), caller_image && caller_interleaved,
-                              d_coef.as<uint32_t>(), stream);
-      else
-        launch_dwt_fwd(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                       img_slot(caller_image), d_coef.as<uint32_t>(), stream, wide);
-      ++last_launches;
-    }
+  if (f.caller_image) enqueue_caller_image();
+  if (f.front == Frame::TRANSCODE) enqueue_transcode_front();
+  else if (f.front == Frame::DWT)
+    enqueue_dwt(true, jobs, d_jobs, img_slot(f.caller_image), f.caller_image && caller_interleaved, d_coef.as<uint32_t>());
   mark(2);
-  if (phase == PHASE_BACK) { mark(3); return; }
-  if (rc_frame) enqueue_rc();
-  enqueue_code();
+  if (f.front == Frame::CODED) { mark(3); return; }
+  if (f.rc) enqueue_rc(f);
+  enqueue_code(f);
   mark(3);
-  };
-  auto rc_times = [&] {
-    if (rq_frame) {
-      const bool eager = h_rq.as<RqState>()->rounds > (uint32_t)RQ_GRAPH_ROUNDS;
-      cudaEventElapsedTime(&rq_ms[0], ev[2], ev[9]); cudaEventElapsedTime(&rq_ms[1], ev[9], ev[10]);
-      if (eager) {
-        float t = 0; cudaEventElapsedTime(&t, rq_ev[0], rq_ev[1]); rq_ms[1] += t;
-        cudaEventElapsedTime(&rq_ms[2], rq_ev[1], rq_ev[2]);
-      } else cudaEventElapsedTime(&rq_ms[2], ev[10], ev[3]);
-      rq_valid = true;
-      return;
-    }
-    if (!rc_frame) return;
-    cudaEventElapsedTime(&rc_ms[0], ev[2], ev[8]); cudaEventElapsedTime(&rc_ms[1], ev[8], ev[9]);
-    cudaEventElapsedTime(&rc_ms[2], ev[9], ev[10]); cudaEventElapsedTime(&rc_ms[3], ev[10], ev[3]);
-  };
-  if (phase == PHASE_FRONT) {
-    enqueue_front();
-    launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches;
-    mark(4);
-    CK(cudaStreamSynchronize(stream));
-    CK(cudaGetLastError());
-    collect(5);
-    status_flags = h_status.as<uint32_t>()[0];
-    if (status_flags & 2u) fail(0x00020001, "mel encoder's buffer is full");
-    if (status_flags & 1u) fail(0x00020005, "block encoder's output slot is full");
-    return 0;
+}
+
+void Encoder::enqueue_code(const Frame& f) {
+  const bool thread_per_block = (serial_block_encoder() && !few_blocks_warp) || max_block_w > 64 || wide;
+  if (thread_per_block)
+    launch_ht_encode_serial(f.code_blocks, f.nb, num_fast_blocks, max_block_w, d_coef.as<uint32_t>(), d_slots.as<uint8_t>(),
+                            d_results.as<EncResult>(), d_tables_enc.as<uint16_t>(), d_status.as<uint32_t>(), stream, wide, &side);
+  else
+    launch_ht_encode(f.code_blocks, f.nb, d_coef.as<uint32_t>(), d_slots.as<uint8_t>(),
+                     d_results.as<EncResult>(), d_tables_enc.as<uint16_t>(), d_status.as<uint32_t>(), stream);
+  last_launches += thread_per_block ? (num_fast_blocks ? 1 : 0) + (num_fast_blocks < f.nb ? 1 : 0) : 1;
+}
+
+void Encoder::check_coder_status() {
+  status_flags = h_status.as<uint32_t>()[0];
+  if (status_flags & 2u) fail(0x00020001, "mel encoder's buffer is full");
+  if (status_flags & 1u) fail(0x00020005, "block encoder's output slot is full");
+}
+
+// rate control: the candidates and the rounds of the selection (rate_ctrl.cu); each round sizes its selection with the
+// packet header kernels, so the block coder's final pass and the headers see the chosen planes in work
+void Encoder::enqueue_rc(const Frame& f) {
+  CK(cudaMemsetAsync(rc.state, 0, sizeof(RcState), stream));
+  launch_rc_prepare(f.blocks, f.nb, d_coef.as<uint32_t>(), rc, stream);
+  mark(8);
+  launch_ht_encode_lengths(f.blocks, f.nb, rc.kc, rc.ncand, max_block_w, d_coef.as<uint32_t>(), rc.cand,
+                           d_tables_enc.as<uint16_t>(), stream);
+  mark(9);
+  launch_rc_hull(f.blocks, f.nb, f.work, d_results.as<EncResult>(), rc, stream);
+  last_launches += 4;
+  if (f.rq) {
+    CK(cudaMemsetAsync(rc.q, 0, sizeof(RqState), stream));
+    launch_rq_init(rc, rq_limit, params.num_comps(), rq_lossless0 && !(f.front == Frame::TRANSCODE && xc_two_pass), stream);
+    ++last_launches;
+    for (int r = 0; r < RQ_GRAPH_ROUNDS; ++r) rq_round(f);
+    rq_final(f);
+    mark(10);
+    return;
   }
-  if (device_headers) {
-    // packet headers, markers and layout by kernels; the host only learns the length (and, for a host buffer, waits
-    // for it before asking for the copy)
-    uint8_t* dev_out;
-    uint64_t cap = out_cap;
-    if (out_on_device) dev_out = out;
-    else {
-      if (d_out.cap < 1024) d_out.reserve(std::max<size_t>(1 << 20, fixed_blob.size() + 64));
-      dev_out = d_out.as<uint8_t>(); cap = std::min<uint64_t>(out_cap, d_out.cap);
-    }
-    uint64_t total = 0;
-    bool grown = false, recode = false;
-    for (int attempt = 0; ; ++attempt) {
-      auto enqueue_all = [&] {
-      if (attempt == 0) { enqueue_front(); launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches; mark(4); mark(5); }
-      else if (recode) {
-        enqueue_code(); launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches;
-        if (rq_frame) CK(cudaEventRecord(rq_ev[2], stream));
-      }
-      if (fixed_blob.size() <= cap) CK(cudaMemcpyAsync(dev_out, d_fixed.p, fixed_blob.size(), cudaMemcpyDeviceToDevice, stream));
-      CK(cudaMemsetAsync(hplan.hscr, 0, hscr_bytes, stream));
-      launch_packet_headers(hplan, code_blocks, d_results.as<EncResult>(), wide ? 62u : 30u, fixed_blob.size(), cap,
-                            tile_mask.empty(), dev_out, d_dst.as<uint64_t>(), stream);
-      if (!tile_mask.empty() && hplan.ntps) { launch_ctrl_copy(h_tpout.p, hplan.tp_out, (size_t)hplan.ntps * 16, stream); ++last_launches; }
-      launch_gather_blocks(d_blocks.as<EncBlock>(), d_results.as<EncResult>(), d_dst.as<uint64_t>(), nb, d_slots.as<uint8_t>(), dev_out, stream);
-      launch_ctrl_copy(h_total.p, hplan.total, 16, stream);
-      last_launches += packet_header_launches(hplan) + 2;
-      mark(6);
-      };
-      // resident form (frame already in HBM, codestream stays there): nothing in the call depends on host data, so
-      // the whole thing replays as a graph (a caller's image is named by the control block the graph copies in,
-      // so its addresses are not part of the key)
-      if (attempt == 0 && planes == nullptr && out_on_device && phase == PHASE_ALL)
-        run_frame({ (uint64_t)(size_t)dev_out, cap, (uint64_t)nb, (uint64_t)num_fast_blocks, (uint64_t)(size_t)d_slots.p, (uint64_t)(size_t)d_coef.p,
-                    rc_frame ? target_bytes : 0, (uint64_t)(size_t)d_rc.p, (uint64_t)(size_t)d_work.p,
-                    rq_frame ? rq_limit : 0, (uint64_t)rq_frame, (uint64_t)(size_t)d_rq.p, (uint64_t)(size_t)d_rcoef.p,
-                    (uint64_t)(size_t)d_rimg.p, (uint64_t)(size_t)d_rq_jobs.p,
-                    (uint64_t)(size_t)img_slot(caller_image), (uint64_t)(caller_image && caller_interleaved) }, enqueue_all);
-      else enqueue_all();
+  rc_size(f, true);
+  for (int r = 0; r < RC_ROUNDS; ++r) {
+    launch_rc_round(f.blocks, f.nb, f.work, d_results.as<EncResult>(), rc, stream);
+    last_launches += 2;
+    rc_size(f, false);
+  }
+  rc_state_out(f);
+  mark(10);
+}
+
+void Encoder::rc_size(const Frame& f, bool first) {
+  launch_packet_header_total(hplan, f.work, d_results.as<EncResult>(), 30u, fixed_blob.size(), true, stream);
+  launch_rc_check(rc, hplan.total, target_bytes, min_bytes, first, stream);
+  last_launches += packet_header_total_launches(hplan) + 1;
+}
+
+void Encoder::rc_state_out(const Frame& f) {
+  launch_ctrl_copy(h_rc.p, rc.state, sizeof(RcState), stream);
+  launch_ctrl_copy(h_rc.as<uint8_t>() + 64, rc.chosen, f.nb, stream);
+  last_launches += 2;
+}
+
+// a round of the quality target: select, reconstruct as the decoder would, synthesise, measure (rate_ctrl.cu).  The
+// synthesis is on 32-bit coefficients: check_target_mse refuses the 64-bit path
+void Encoder::rq_round(const Frame& f) {
+  launch_rq_select(d_blocks.as<EncBlock>(), f.blocks, f.nb, f.work, d_results.as<EncResult>(), d_coef.as<uint32_t>(),
+                   d_rcoef.as<uint32_t>(), rc, stream);
+  last_launches += 3;
+  enqueue_dwt(false, rq_jobs, d_rq_jobs, scratch_slot(), false, d_rcoef.as<uint32_t>());
+  launch_rq_measure(scratch_slot(), img_slot(f.caller_image), rq_image, rc, stream);
+  last_launches += 2;
+}
+
+void Encoder::rq_final(const Frame& f) {
+  launch_rq_final(f.blocks, f.nb, f.work, d_results.as<EncResult>(), rc, stream);
+  launch_ctrl_copy(h_rq.p, rc.q, sizeof(RqState), stream);
+  launch_ctrl_copy(h_rc.as<uint8_t>() + 64, rc.chosen, f.nb, stream);
+  last_launches += 3;
+}
+
+// after the frame's rounds: the rare selection that still does not fit goes on eagerly; true = it changed
+bool Encoder::rc_settle(const Frame& f) {
+  if (f.rq) {
+    if (h_rq.as<RqState>()->done) return false;
+    CK(cudaEventRecord(rq_ev[0], stream));
+    // the bracket closes within RQ_BODY_ROUNDS + 34 rounds (rq_update_kernel); one synchronisation per round
+    while (!h_rq.as<RqState>()->done) {
+      rq_round(f);
+      launch_ctrl_copy(h_rq.p, rc.q, sizeof(RqState), stream); ++last_launches;
       CK(cudaStreamSynchronize(stream));
-      CK(cudaGetLastError());
-      status_flags = h_status.as<uint32_t>()[0];
-      if (status_flags & 2u) fail(0x00020001, "mel encoder's buffer is full");
-      if (status_flags & 1u) fail(0x00020005, "block encoder's output slot is full");
-      if (attempt == 0 && rc_settle()) { recode = true; continue; }     // code and lay out the settled selection
-      recode = false;
-      total = h_total.as<uint64_t>()[0];
-      if (h_total.as<uint64_t>()[1] == 0) break;
-      // did not fit: the caller's buffer is too small, or (host output) the staging buffer has to grow once
-      if (total > out_cap || out_on_device || grown)
-        fail(0x000B0030, "output buffer too small: need %zu bytes, have %zu", (size_t)total, out_cap);
-      grown = true;
-      d_out.reserve(total + 64); dev_out = d_out.as<uint8_t>(); cap = std::min<uint64_t>(out_cap, d_out.cap);
     }
-    host_ms = 0;
-    last_tileparts.clear();
-    if (!tile_mask.empty())
-      for (uint32_t i = 0; i < hplan.ntps; ++i)
-        last_tileparts.push_back(TilePartOut{ h_tp_tile[i], h_tpout.as<uint64_t>()[2 * i], (uint32_t)h_tpout.as<uint64_t>()[2 * i + 1] });
-    if (!out_on_device) CK(cudaMemcpyAsync(out, dev_out, total, cudaMemcpyDeviceToHost, stream));
-    mark(7);
-    CK(cudaStreamSynchronize(stream));
-    collect(8);
-    rc_times();
-    CK(cudaGetLastError());
-    std::fill(line_cur.begin(), line_cur.end(), 0u); cur_comp = 0; lines_done = false;
-    return (size_t)total;
+    rq_final(f);
+    CK(cudaEventRecord(rq_ev[1], stream));
+    return true;
   }
-  enqueue_front();
+  if (!f.rc || h_rc.as<RcState>()->done) return false;
+  for (int i = 0; !h_rc.as<RcState>()->done; ++i) {
+    // every round over the target strictly lowers the selected body (rc_check_kernel), so there are at most as many
+    // rounds as distinct selections: one more hull segment per block and round at the very worst
+    if ((uint64_t)i > (uint64_t)f.nb * rc.kc + 2)
+      fail(0x000B003A, "rate control did not settle on a selection that fits the target (internal error)");
+    launch_rc_round(f.blocks, f.nb, f.work, d_results.as<EncResult>(), rc, stream);
+    last_launches += 2;
+    rc_size(f, false);
+    rc_state_out(f);
+    CK(cudaStreamSynchronize(stream));
+  }
+  return true;
+}
+
+// packet headers, markers and layout by kernels; the host only learns the length (and, for a host buffer, waits for it
+// before asking for the copy)
+size_t Encoder::finish_device(const Frame& f, uint8_t* out, size_t out_cap, bool out_on_device) {
+  uint8_t* dev_out;
+  uint64_t cap = out_cap;
+  if (out_on_device) dev_out = out;
+  else {
+    if (d_out.cap < 1024) d_out.reserve(std::max<size_t>(1 << 20, fixed_blob.size() + 64));
+    dev_out = d_out.as<uint8_t>(); cap = std::min<uint64_t>(out_cap, d_out.cap);
+  }
+  auto sync = [&] {
+    CK(cudaStreamSynchronize(stream));
+    CK(cudaGetLastError());
+    check_coder_status();
+  };
+  auto enqueue = [&] {
+    enqueue_front(f);
+    launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches;
+    mark(4); mark(5);
+    enqueue_device_layout(f, dev_out, cap);
+  };
+  // resident form (frame already in HBM, codestream stays there): nothing in the call depends on host data, so the
+  // whole thing replays as a graph (a caller's image is named by the control block the graph copies in, so its
+  // addresses are not part of the key)
+  if (f.graph)
+    run_frame({ (uint64_t)(size_t)dev_out, cap, (uint64_t)f.nb, (uint64_t)num_fast_blocks, (uint64_t)(size_t)d_slots.p, (uint64_t)(size_t)d_coef.p,
+                f.rc ? target_bytes : 0, (uint64_t)(size_t)d_rc.p, (uint64_t)(size_t)d_work.p,
+                f.rq ? rq_limit : 0, (uint64_t)f.rq, (uint64_t)(size_t)d_rq.p, (uint64_t)(size_t)d_rcoef.p,
+                (uint64_t)(size_t)d_rimg.p, (uint64_t)(size_t)d_rq_jobs.p,
+                (uint64_t)(size_t)img_slot(f.caller_image), (uint64_t)(f.caller_image && caller_interleaved) }, enqueue);
+  else enqueue();
+  sync();
+  if (rc_settle(f)) {                  // code and lay out the settled selection
+    enqueue_code(f); launch_ctrl_copy(h_status.p, d_status.p, 16, stream); ++last_launches;
+    if (f.rq) CK(cudaEventRecord(rq_ev[2], stream));
+    enqueue_device_layout(f, dev_out, cap);
+    sync();
+  }
+  // did not fit: the caller's buffer is too small, or (host output) the staging buffer has to grow once
+  for (bool grown = false; h_total.as<uint64_t>()[1] != 0; grown = true) {
+    const size_t need = (size_t)h_total.as<uint64_t>()[0];
+    if (need > out_cap || out_on_device || grown)
+      fail(0x000B0030, "output buffer too small: need %zu bytes, have %zu", need, out_cap);
+    d_out.reserve(need + 64); dev_out = d_out.as<uint8_t>(); cap = std::min<uint64_t>(out_cap, d_out.cap);
+    enqueue_device_layout(f, dev_out, cap);
+    sync();
+  }
+  host_ms = 0;
+  last_tileparts.clear();
+  if (!tile_mask.empty())
+    for (uint32_t i = 0; i < hplan.ntps; ++i)
+      last_tileparts.push_back(TilePartOut{ h_tp_tile[i], h_tpout.as<uint64_t>()[2 * i], (uint32_t)h_tpout.as<uint64_t>()[2 * i + 1] });
+  return end_frame(f, out, dev_out, (size_t)h_total.as<uint64_t>()[0], out_on_device);
+}
+
+void Encoder::enqueue_device_layout(const Frame& f, uint8_t* dev_out, uint64_t cap) {
+  if (fixed_blob.size() <= cap) CK(cudaMemcpyAsync(dev_out, d_fixed.p, fixed_blob.size(), cudaMemcpyDeviceToDevice, stream));
+  CK(cudaMemsetAsync(hplan.hscr, 0, hscr_bytes, stream));
+  launch_packet_headers(hplan, f.code_blocks, d_results.as<EncResult>(), wide ? 62u : 30u, fixed_blob.size(), cap,
+                        tile_mask.empty(), dev_out, d_dst.as<uint64_t>(), stream);
+  if (!tile_mask.empty() && hplan.ntps) { launch_ctrl_copy(h_tpout.p, hplan.tp_out, (size_t)hplan.ntps * 16, stream); ++last_launches; }
+  launch_gather_blocks(d_blocks.as<EncBlock>(), d_results.as<EncResult>(), d_dst.as<uint64_t>(), f.nb, d_slots.as<uint8_t>(), dev_out, stream);
+  launch_ctrl_copy(h_total.p, hplan.total, 16, stream);
+  last_launches += packet_header_launches(hplan) + 2;
+  mark(6);
+}
+
+// the host writer's frame: packets with their headers, tile-parts, and everything that is not code-block data (blob)
+// with the pieces that place it in the codestream
+struct Encoder::HostLayout {
+  struct Pkt { PacketRef ref; std::vector<uint8_t> hdr; uint32_t hdr_len, body; };
+  struct TilePart { uint32_t tile, first, count, tp_idx, tp_cnt; uint64_t bytes; };
+  struct Piece { size_t src, dst; uint32_t len; };
+  std::vector<Pkt> pkts;
+  std::vector<TilePart> tps;
+  std::vector<uint8_t> blob;
+  std::vector<Piece> pieces;
+};
+
+// packet headers and the final layout on the host (with a target: at the planes the selection chose), assembled on
+// the device with one copy out
+size_t Encoder::finish_host(const Frame& f, uint8_t* out, size_t out_cap, bool out_on_device) {
+  const uint32_t nb = f.nb;
+  enqueue_front(f);
   if (nb) launch_ctrl_copy(h_results.p, d_results.p, (size_t)nb * sizeof(EncResult), stream);
   launch_ctrl_copy(h_status.p, d_status.p, 16, stream);
   last_launches += nb ? 2 : 1;
@@ -1058,22 +1092,52 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
   CK(cudaStreamSynchronize(stream));
   auto host_t0 = std::chrono::steady_clock::now();
   CK(cudaGetLastError());
-  status_flags = h_status.as<uint32_t>()[0];
-  if (status_flags & 2u) fail(0x00020001, "mel encoder's buffer is full");
-  if (status_flags & 1u) fail(0x00020005, "block encoder's output slot is full");
-  if (rc_settle()) {
-    enqueue_code();
-    if (rq_frame) CK(cudaEventRecord(rq_ev[2], stream));
+  check_coder_status();
+  if (rc_settle(f)) {
+    enqueue_code(f);
+    if (f.rq) CK(cudaEventRecord(rq_ev[2], stream));
     launch_ctrl_copy(h_results.p, d_results.p, (size_t)nb * sizeof(EncResult), stream); ++last_launches;
     CK(cudaStreamSynchronize(stream));
     CK(cudaGetLastError());
   }
+  HostLayout hl;
+  host_packets(f, hl);
+  const size_t total = host_markers(hl);
+  if (total > out_cap) fail(0x000B0030, "output buffer too small: need %zu bytes, have %zu", total, out_cap);
+  const std::vector<uint8_t>& blob = hl.blob;
+  const std::vector<HostLayout::Piece>& pieces = hl.pieces;
+  uint8_t* dev_out;
+  if (out_on_device) dev_out = out; else { d_out.reserve(total + 64); dev_out = d_out.as<uint8_t>(); }
+  h_hdr.reserve(blob.size() + 64); memcpy(h_hdr.p, blob.data(), blob.size());
+  host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
+  mark(5);
+  d_hdr.reserve(blob.size() + 64);
+  launch_ctrl_copy(d_hdr.p, h_hdr.p, blob.size(), stream);
+  h_pieces.reserve(pieces.size() * sizeof(CopyPiece)); d_pieces.reserve(pieces.size() * sizeof(CopyPiece));
+  CopyPiece* cp = h_pieces.as<CopyPiece>();
+  uint32_t max_piece = 0;
+  for (size_t i = 0; i < pieces.size(); ++i) {
+    cp[i].src_off = pieces[i].src; cp[i].dst_off = pieces[i].dst; cp[i].len = pieces[i].len; cp[i].src_sel = 1;
+    max_piece = std::max(max_piece, cp[i].len);
+  }
+  launch_ctrl_copy(d_pieces.p, h_pieces.p, pieces.size() * sizeof(CopyPiece), stream);
+  if (nb) launch_ctrl_copy(d_dst.p, h_dst.p, (size_t)nb * 8, stream);
+  last_launches += (blob.size() ? 1 : 0) + (pieces.empty() ? 0 : 1) + (nb ? 1 : 0);
+  launch_gather_blocks(f.code_blocks, d_results.as<EncResult>(), d_dst.as<uint64_t>(), nb,
+                       d_slots.as<uint8_t>(), dev_out, stream);
+  launch_assemble(d_pieces.as<CopyPiece>(), (uint32_t)pieces.size(), max_piece, d_slots.as<uint8_t>(), d_hdr.as<uint8_t>(), dev_out, stream);
+  last_launches += 2;
+  mark(6);
+  return end_frame(f, out, dev_out, total, out_on_device);
+}
 
-  // 3. packet headers and final layout on the host (with a target: at the planes the selection chose)
+// the blocks' records from the coder's results, the packet sequence of every tile-part and the packet headers
+void Encoder::host_packets(const Frame& f, HostLayout& hl) {
+  const uint32_t nb = f.nb;
   const EncResult* res = h_results.as<EncResult>();
-  const uint8_t* chosen = rc_frame ? h_rc.as<uint8_t>() + 64 : nullptr;
+  const uint8_t* chosen = f.rc ? h_rc.as<uint8_t>() + 64 : nullptr;
   std::vector<EncBlock> xb;                // a transcode's per-frame start planes
-  if (phase == PHASE_TRANSCODE && nb) {
+  if (f.front == Frame::TRANSCODE && nb) {
     xb.resize(nb);
     CK(cudaMemcpy(xb.data(), d_xblocks.p, (size_t)nb * sizeof(EncBlock), cudaMemcpyDeviceToHost));
   }
@@ -1085,83 +1149,79 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     cb.num_passes = len ? 1 : 0;
     cb.missing_msbs = len ? (uint8_t)((wide ? 62u : 30u) - hb[b].p - (chosen ? chosen[b] : 0u)) : 0;
   }
-  struct Pkt { PacketRef ref; std::vector<uint8_t> hdr; uint32_t hdr_len, body; };
-  struct TilePart { uint32_t tile, first, count, tp_idx, tp_cnt; uint64_t bytes; };
-  std::vector<Pkt> pkts;
-  std::vector<TilePart> tps;
-  {
-    std::vector<PacketRef> seq; std::vector<uint32_t> tp_first, tp_index;
-    uint32_t tp_total = 0;
-    for (uint32_t t = 0; t < (uint32_t)layout.tiles.size(); ++t) {
-      if (!tile_wanted(t)) continue;
-      layout.packet_sequence(t, seq, tp_first, &tp_index, &tp_total);
-      size_t base = pkts.size();
-      for (const PacketRef& pr : seq) { pkts.emplace_back(); pkts.back().ref = pr; pkts.back().hdr_len = pkts.back().body = 0; }
-      for (size_t i = 0; i < tp_first.size(); ++i) {
-        TilePart tp; tp.tile = t; tp.first = (uint32_t)(base + tp_first[i]);
-        uint32_t end = (i + 1 < tp_first.size()) ? tp_first[i + 1] : (uint32_t)seq.size();
-        tp.count = end - tp_first[i]; tp.tp_idx = tp_index[i]; tp.tp_cnt = tp_total;
-        tp.bytes = 0;
-        tps.push_back(tp);
-      }
+  std::vector<HostLayout::Pkt>& pkts = hl.pkts;
+  std::vector<PacketRef> seq; std::vector<uint32_t> tp_first, tp_index;
+  uint32_t tp_total = 0;
+  for (uint32_t t = 0; t < (uint32_t)layout.tiles.size(); ++t) {
+    if (!tile_wanted(t)) continue;
+    layout.packet_sequence(t, seq, tp_first, &tp_index, &tp_total);
+    size_t base = pkts.size();
+    for (const PacketRef& pr : seq) { pkts.emplace_back(); pkts.back().ref = pr; pkts.back().hdr_len = pkts.back().body = 0; }
+    for (size_t i = 0; i < tp_first.size(); ++i) {
+      HostLayout::TilePart tp; tp.tile = t; tp.first = (uint32_t)(base + tp_first[i]);
+      uint32_t end = (i + 1 < tp_first.size()) ? tp_first[i + 1] : (uint32_t)seq.size();
+      tp.count = end - tp_first[i]; tp.tp_idx = tp_index[i]; tp.tp_cnt = tp_total;
+      tp.bytes = 0;
+      hl.tps.push_back(tp);
     }
   }
-  {
-    // packet headers are independent of each other: a few host threads share them (largest first)
-    std::vector<uint32_t> order(pkts.size());
-    for (uint32_t i = 0; i < order.size(); ++i) order[i] = i;
-    auto weight = [&](uint32_t i) {
-      const ResGeom& rg = layout.res_of(pkts[i].ref); const PrecinctGeom& pc = rg.precincts[pkts[i].ref.precinct];
-      uint32_t n = 0; for (int b = 0; b < 4; ++b) n += pc.cb_idx[b].w * pc.cb_idx[b].h; return n;
-    };
-    std::vector<uint32_t> wt(pkts.size());
-    for (uint32_t i = 0; i < wt.size(); ++i) wt[i] = weight(i);
-    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return wt[a] > wt[b]; });
-    std::atomic<uint32_t> next(0);
-    auto work = [&]() {
-      for (;;) {
-        uint32_t k = next.fetch_add(1);
-        if (k >= order.size()) break;
-        Pkt& pk = pkts[order[k]];
-        const ResGeom& rg = layout.res_of(pk.ref);
-        pk.hdr.reserve(64 + wt[order[k]] * 4);
-        pk.body = write_packet_header(rg, rg.precincts[pk.ref.precinct], coded.data(), pk.hdr);
-        pk.hdr_len = (uint32_t)pk.hdr.size();
-      }
-    };
-    uint32_t nthreads = (uint32_t)std::min<size_t>(std::min<size_t>(host_threads, pkts.size()), 16);
-    if (nb < 2048 || nthreads <= 1) work();
-    else {
-      std::vector<std::thread> th;
-      for (uint32_t i = 1; i < nthreads; ++i) th.emplace_back(work);
-      work();
-      for (auto& t : th) t.join();
+  // packet headers are independent of each other: a few host threads share them (largest first)
+  std::vector<uint32_t> order(pkts.size());
+  for (uint32_t i = 0; i < order.size(); ++i) order[i] = i;
+  auto weight = [&](uint32_t i) {
+    const ResGeom& rg = layout.res_of(pkts[i].ref); const PrecinctGeom& pc = rg.precincts[pkts[i].ref.precinct];
+    uint32_t n = 0; for (int b = 0; b < 4; ++b) n += pc.cb_idx[b].w * pc.cb_idx[b].h; return n;
+  };
+  std::vector<uint32_t> wt(pkts.size());
+  for (uint32_t i = 0; i < wt.size(); ++i) wt[i] = weight(i);
+  std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return wt[a] > wt[b]; });
+  std::atomic<uint32_t> next(0);
+  auto work = [&]() {
+    for (;;) {
+      uint32_t k = next.fetch_add(1);
+      if (k >= order.size()) break;
+      HostLayout::Pkt& pk = pkts[order[k]];
+      const ResGeom& rg = layout.res_of(pk.ref);
+      pk.hdr.reserve(64 + wt[order[k]] * 4);
+      pk.body = write_packet_header(rg, rg.precincts[pk.ref.precinct], coded.data(), pk.hdr);
+      pk.hdr_len = (uint32_t)pk.hdr.size();
     }
+  };
+  uint32_t nthreads = (uint32_t)std::min<size_t>(std::min<size_t>(host_threads, pkts.size()), 16);
+  if (nb < 2048 || nthreads <= 1) work();
+  else {
+    std::vector<std::thread> th;
+    for (uint32_t i = 1; i < nthreads; ++i) th.emplace_back(work);
+    work();
+    for (auto& t : th) t.join();
   }
-  for (TilePart& tp : tps)
+  for (HostLayout::TilePart& tp : hl.tps)
     for (uint32_t q = 0; q < tp.count; ++q) tp.bytes += pkts[tp.first + q].hdr_len + pkts[tp.first + q].body;
-  // marker bytes: main header [+ TLM], SOT+SOD per tile-part, EOC
-  std::vector<uint8_t> blob;               // everything that is not code-block data, in order
-  struct Piece { size_t src, dst; uint32_t len; };
-  std::vector<Piece> pieces;
+}
+
+// marker bytes (main header [+ TLM], SOT+SOD per tile-part, EOC) and packet headers into the blob, the pieces that
+// place it and each block's offset (h_dst); returns the codestream's length
+size_t Encoder::host_markers(HostLayout& hl) {
+  std::vector<uint8_t>& blob = hl.blob;
+  std::vector<HostLayout::Piece>& pieces = hl.pieces;
   uint64_t pos = 0;
   auto add_piece = [&](size_t src, uint32_t len) {
     if (!pieces.empty() && pieces.back().src + pieces.back().len == src && pieces.back().dst + pieces.back().len == pos)
       pieces.back().len += len;
-    else pieces.push_back(Piece{ src, (size_t)pos, len });
+    else pieces.push_back(HostLayout::Piece{ src, (size_t)pos, len });
     pos += len;
   };
   const bool partial = !tile_mask.empty();       // tile-parts only: the writer rank adds main header, TLM and EOC
   if (!partial) blob = main_header;
   last_tileparts.clear();
-  if (P.need_tlm && !partial) {
-    if (4 + 6 * tps.size() > 65535) fail(0x000500B1, "too many tile-parts for one TLM marker segment");
-    put_u16(blob, M_TLM); put_u16(blob, (uint32_t)(4 + 6 * tps.size())); put_u8(blob, 0); put_u8(blob, 0x60);
-    for (const TilePart& tp : tps) { put_u16(blob, tp.tile); put_u32(blob, (uint32_t)(tp.bytes + 14)); }
+  if (params.need_tlm && !partial) {
+    if (4 + 6 * hl.tps.size() > 65535) fail(0x000500B1, "too many tile-parts for one TLM marker segment");
+    put_u16(blob, M_TLM); put_u16(blob, (uint32_t)(4 + 6 * hl.tps.size())); put_u8(blob, 0); put_u8(blob, 0x60);
+    for (const HostLayout::TilePart& tp : hl.tps) { put_u16(blob, tp.tile); put_u32(blob, (uint32_t)(tp.bytes + 14)); }
   }
   if (!blob.empty()) add_piece(0, (uint32_t)blob.size());
   uint64_t* dst = h_dst.as<uint64_t>();
-  for (const TilePart& tp : tps) {
+  for (const HostLayout::TilePart& tp : hl.tps) {
     size_t s = blob.size();
     last_tileparts.push_back(TilePartOut{ tp.tile, pos, (uint32_t)(tp.bytes + 14) });
     put_u16(blob, M_SOT); put_u16(blob, 10); put_u16(blob, tp.tile); put_u32(blob, (uint32_t)(tp.bytes + 14));
@@ -1169,7 +1229,7 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     put_u16(blob, M_SOD);
     add_piece(s, 14);
     for (uint32_t q = 0; q < tp.count; ++q) {
-      const Pkt& k = pkts[tp.first + q];
+      const HostLayout::Pkt& k = hl.pkts[tp.first + q];
       size_t hs = blob.size();
       blob.insert(blob.end(), k.hdr.begin(), k.hdr.end());
       add_piece(hs, k.hdr_len);
@@ -1189,41 +1249,35 @@ size_t Encoder::encode(const void* const* planes, const uint32_t* strides, bool 
     }
   }
   if (!partial) { size_t s = blob.size(); put_u16(blob, M_EOC); add_piece(s, 2); }
-  const size_t total = (size_t)pos;
-  if (total > out_cap) fail(0x000B0030, "output buffer too small: need %zu bytes, have %zu", total, out_cap);
+  return (size_t)pos;
+}
 
-  // 4. assemble on the device, one copy out
-  uint8_t* dev_out;
-  if (out_on_device) dev_out = out; else { d_out.reserve(total + 64); dev_out = d_out.as<uint8_t>(); }
-  h_hdr.reserve(blob.size() + 64); memcpy(h_hdr.p, blob.data(), blob.size());
-  host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
-  mark(5);
-  d_hdr.reserve(blob.size() + 64);
-  launch_ctrl_copy(d_hdr.p, h_hdr.p, blob.size(), stream);
-  h_pieces.reserve(pieces.size() * sizeof(CopyPiece)); d_pieces.reserve(pieces.size() * sizeof(CopyPiece));
-  CopyPiece* cp = h_pieces.as<CopyPiece>();
-  uint32_t max_piece = 0;
-  for (size_t i = 0; i < pieces.size(); ++i) {
-    cp[i].src_off = pieces[i].src; cp[i].dst_off = pieces[i].dst; cp[i].len = pieces[i].len; cp[i].src_sel = 1;
-    max_piece = std::max(max_piece, cp[i].len);
-  }
-  launch_ctrl_copy(d_pieces.p, h_pieces.p, pieces.size() * sizeof(CopyPiece), stream);
-  if (nb) launch_ctrl_copy(d_dst.p, h_dst.p, (size_t)nb * 8, stream);
-  last_launches += (blob.size() ? 1 : 0) + (pieces.empty() ? 0 : 1) + (nb ? 1 : 0);
-  launch_gather_blocks(code_blocks, d_results.as<EncResult>(), d_dst.as<uint64_t>(), nb,
-                       d_slots.as<uint8_t>(), dev_out, stream);
-  launch_assemble(d_pieces.as<CopyPiece>(), (uint32_t)pieces.size(), max_piece, d_slots.as<uint8_t>(), d_hdr.as<uint8_t>(), dev_out, stream);
-  last_launches += 2;
-  mark(6);
+// the end of both finishing paths: the codestream to a host buffer, the stage times, the line front end reset
+size_t Encoder::end_frame(const Frame& f, uint8_t* out, const uint8_t* dev_out, size_t total, bool out_on_device) {
   if (!out_on_device) CK(cudaMemcpyAsync(out, dev_out, total, cudaMemcpyDeviceToHost, stream));
   mark(7);
   CK(cudaStreamSynchronize(stream));
   collect(8);
-  rc_times();
+  rc_times(f);
   CK(cudaGetLastError());
-  // reset the line front end for the next frame
   std::fill(line_cur.begin(), line_cur.end(), 0u); cur_comp = 0; lines_done = false;
   return total;
+}
+
+void Encoder::rc_times(const Frame& f) {
+  if (f.rq) {
+    const bool eager = h_rq.as<RqState>()->rounds > (uint32_t)RQ_GRAPH_ROUNDS;
+    cudaEventElapsedTime(&rq_ms[0], ev[2], ev[9]); cudaEventElapsedTime(&rq_ms[1], ev[9], ev[10]);
+    if (eager) {
+      float t = 0; cudaEventElapsedTime(&t, rq_ev[0], rq_ev[1]); rq_ms[1] += t;
+      cudaEventElapsedTime(&rq_ms[2], rq_ev[1], rq_ev[2]);
+    } else cudaEventElapsedTime(&rq_ms[2], ev[10], ev[3]);
+    rq_valid = true;
+    return;
+  }
+  if (!f.rc) return;
+  cudaEventElapsedTime(&rc_ms[0], ev[2], ev[8]); cudaEventElapsedTime(&rc_ms[1], ev[8], ev[9]);
+  cudaEventElapsedTime(&rc_ms[2], ev[9], ev[10]); cudaEventElapsedTime(&rc_ms[3], ev[10], ev[3]);
 }
 
 //------------------------------------------------------------------------------------------
@@ -1545,7 +1599,7 @@ void Decoder::enqueue_blocks(const BlockFrame& f, const DecDyn* hy, const uint8_
 
 uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool caller_image) {
   const Params& P = params;
-  uint32_t nc = P.num_comps(), es = esize_of(img_type), D = P.num_decomps;
+  uint32_t nc = P.num_comps(), es = esize_of(img_type);
   last_launches = 0;
   // codestream to the device while the host parses packet headers
   mark(0);
@@ -1591,19 +1645,7 @@ uint32_t Decoder::decode(void* const* planes, const uint32_t* strides, bool call
   mark(3);
   if (nb) { launch_ctrl_copy(h_bstatus.p, d_bstatus.p, (size_t)nb * 4, stream); ++last_launches; }
   if (caller_image) enqueue_caller_image();
-  // synthesis, coarsest level first
-  for (size_t li = jobs.size(); li-- > 0; )
-    for (const JobGroup& g : jobs[li]) {
-      if (g.stream)
-        launch_dwt_inv_stream(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                              g.first, img_type, img_slot(caller_image), caller_image && caller_interleaved,
-                              d_coef.as<uint32_t>(), stream);
-      else
-        launch_dwt_inv(d_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                       img_slot(caller_image), d_coef.as<uint32_t>(), stream, wide);
-      ++last_launches;
-    }
-  (void)D;
+  enqueue_dwt(false, jobs, d_jobs, img_slot(caller_image), caller_image && caller_interleaved, d_coef.as<uint32_t>());
   mark(4);
   if (planes) {
     for (uint32_t c = 0; c < nc; ++c) {
@@ -1721,16 +1763,8 @@ void Encoder::enqueue_transcode_front() {
   }
   if (rq_on() && rq_planned) {
     D.enqueue_blocks(xc_source, h_xdyn.as<DecDyn>(), xc_cs, d_rcoef.as<uint32_t>(), stream, &side, last_launches);
-    for (size_t li = rq_jobs.size(); li-- > 0; )
-      for (const JobGroup& g : rq_jobs[li]) {
-        if (g.stream)
-          launch_dwt_inv_stream(d_rq_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                                g.first, img_type, img_slot(false), false, d_rcoef.as<uint32_t>(), stream);
-        else
-          launch_dwt_inv(d_rq_jobs.as<DwtJob>() + g.dev_off, (uint32_t)g.jobs.size(), g.ctas, g.reversible, g.ncomp,
-                         img_slot(false), d_rcoef.as<uint32_t>(), stream, false);
-        ++last_launches;
-      }
+    // 32-bit coefficients: transcode_parse refuses an input on the 64-bit path
+    enqueue_dwt(false, rq_jobs, d_rq_jobs, img_slot(false), false, d_rcoef.as<uint32_t>());
   }
   D.enqueue_blocks(xc_coded, D.h_dyn.as<DecDyn>(), xc_cs, d_coef.as<uint32_t>(), stream, &side, last_launches);
   if (nb) { launch_ctrl_copy(D.h_bstatus.p, D.d_bstatus.p, (size_t)nb * 4, stream); ++last_launches; }
@@ -1766,10 +1800,8 @@ size_t Encoder::transcode(const uint8_t* j2c, size_t len, bool on_device, uint8_
   if (on_device) xc_cs = j2c;
   else { D.d_cs.reserve(len + 64); xc_cs = D.d_cs.as<uint8_t>(); }
   const float parse_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  phase = PHASE_TRANSCODE;
-  size_t n = 0;
-  try { n = encode(nullptr, nullptr, false, out, out_cap, out_on_device); } catch (...) { phase = PHASE_ALL; throw; }
-  phase = PHASE_ALL;
+  const Frame f = begin_frame(Frame::TRANSCODE, true);
+  const size_t n = device_headers ? finish_device(f, out, out_cap, out_on_device) : finish_host(f, out, out_cap, out_on_device);
   host_ms = parse_ms;
   const uint32_t* bs = D.h_bstatus.as<uint32_t>();
   for (uint32_t b = 0; b < nb; ++b)

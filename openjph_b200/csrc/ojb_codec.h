@@ -29,6 +29,12 @@ struct Timings { float h2d_ms = 0, kernels_ms = 0, host_ms = 0, d2h_ms = 0; };
 
 // sample container of the image buffers handed to / returned by the frame calls
 enum SampleType : uint32_t { ST_U8 = 0, ST_U16 = 1, ST_I32 = 2 };
+inline uint32_t esize_of(uint32_t st) { return st == ST_U8 ? 1u : (st == ST_U16 ? 2u : 4u); }
+
+// the HT tables the block encoders (enc) or decoders read, packed as ojb_kernels.h describes them, into dev
+void upload_ht_tables(bool enc, DeviceBuf& dev);
+// a code-block's slot in the encoder's arena: its worst-case bytes, a multiple of 16
+uint32_t enc_slot_cap(uint32_t w, uint32_t h, uint32_t K_max, bool wide);
 
 class CodecBase {
 public:
@@ -98,6 +104,10 @@ public:
   DeviceBuf d_jobs;
   // the analysis (forward) or synthesis jobs of the geometry into out, uploaded to dev (the codec's own: jobs, d_jobs)
   void build_dwt_jobs(bool forward, std::vector<std::vector<JobGroup>>& out, DeviceBuf& dev);
+  // every level of groups (uploaded to dev) between the image img and the arena coef: analysis from the finest level
+  // down, synthesis from the coarsest up
+  void enqueue_dwt(bool forward, const std::vector<std::vector<JobGroup>>& groups, DeviceBuf& dev, const ImgComp* img,
+                   bool interleaved, uint32_t* coef);
   // one image over several GPUs (ojb_shard.cpp): this object works on the tiles whose mask byte is set (empty =
   // all tiles).  The geometry, arenas and block tables stay those of the whole image, so Isot, canvas coordinates
   // and byte offsets are the single-encoder ones; DWT jobs, code-blocks and packets of the other tiles are skipped.
@@ -143,12 +153,45 @@ public:
   // (caller_image: described by use_caller_image)
   size_t encode(const void* const* planes, const uint32_t* strides, bool caller_image,
                 uint8_t* out, size_t out_cap, bool out_on_device);
+  // row regions (ojb_shard.cpp): the frame call split at the point where code-block bytes change hands.  encode_front:
+  // this rank's transform and block coding of the image in d_image; encode_back, on the writer once every rank's blocks
+  // sit in its slots: packet headers, markers and layout into out (device memory)
+  void encode_front();
+  size_t encode_back(uint8_t* out, size_t out_cap);
   uint32_t status_flags = 0;
-  // row regions (ojb_shard.cpp): the frame call split at the point where code-block bytes change hands
-  // PHASE_TRANSCODE: the frame's coefficients come from an input codestream's code-blocks (transcode) instead of the
-  // forward DWT; everything after the transform runs as in PHASE_ALL
-  enum Phase : uint32_t { PHASE_ALL = 0, PHASE_FRONT = 1, PHASE_BACK = 2, PHASE_TRANSCODE = 3 };
-  uint32_t phase = PHASE_ALL;
+  // The stages of a frame call.  Frame holds what the entry point chose for this frame: where the coefficients come
+  // from (front: the forward DWT, a transcode's block decoders, or nothing -- encode_back's blocks are coded already),
+  // whether a target selects the coded planes, and the block arrays the stages read.
+  struct Frame {
+    enum Front : uint8_t { DWT, TRANSCODE, CODED } front = DWT;
+    bool caller_image = false;
+    bool graph = false;                  // the device work may be captured and replayed as a graph (resident form)
+    bool rc = false, rq = false;         // a size or a quality target selects each block's plane
+    uint32_t nb = 0;
+    const EncBlock* blocks = nullptr;    // where each block starts (a transcode: at the input's plane)
+    const EncBlock* code_blocks = nullptr;   // what the block coder codes: blocks, or with a target the selection in work
+    EncBlock* work = nullptr;
+  };
+  Frame begin_frame(Frame::Front front, bool targets, bool caller_image = false, const void* const* planes = nullptr,
+                    const uint32_t* strides = nullptr);
+  void upload_planes(const void* const* planes, const uint32_t* strides);   // host planes -> d_image, on stream
+  void enqueue_front(const Frame& f);
+  void enqueue_code(const Frame& f);
+  void enqueue_rc(const Frame& f);     // a target's candidates and the selection rounds inside the frame's graph
+  void rc_size(const Frame& f, bool first);
+  void rc_state_out(const Frame& f);
+  void rq_round(const Frame& f);
+  void rq_final(const Frame& f);
+  bool rc_settle(const Frame& f);
+  void check_coder_status();
+  size_t finish_device(const Frame& f, uint8_t* out, size_t out_cap, bool out_on_device);
+  void enqueue_device_layout(const Frame& f, uint8_t* dev_out, uint64_t cap);
+  size_t finish_host(const Frame& f, uint8_t* out, size_t out_cap, bool out_on_device);
+  struct HostLayout;
+  void host_packets(const Frame& f, HostLayout& hl);
+  size_t host_markers(HostLayout& hl);
+  size_t end_frame(const Frame& f, uint8_t* out, const uint8_t* dev_out, size_t total, bool out_on_device);
+  void rc_times(const Frame& f);
   // line-based front end (ojph::codestream::exchange): lines go to a pinned frame
   PinnedBuf h_frame;
   std::vector<uint32_t> line_cur;
@@ -193,6 +236,7 @@ public:
   uint32_t rc_kc = 0;
   float rc_ms[4] = {0, 0, 0, 0};       // last frame: distortion, candidate lengths, selection, final encode
   void set_target(uint64_t bytes);
+  void check_target_size(uint64_t bytes) const;
   uint64_t min_size_of_geometry() const;
   void plan_rate_control();
   bool rc_on() const { return target_bytes != 0; }
@@ -238,7 +282,6 @@ public:
   size_t transcode(const uint8_t* j2c, size_t len, bool on_device, uint8_t* out, size_t out_cap, bool out_on_device);
   void transcode_parse(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type);
   void enqueue_transcode_front();
-  const EncBlock* frame_blocks() { return phase == PHASE_TRANSCODE ? d_xblocks.as<EncBlock>() : d_blocks.as<EncBlock>(); }
 };
 
 struct FrameInfo {

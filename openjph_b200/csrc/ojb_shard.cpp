@@ -143,8 +143,6 @@ struct NcclComm : Comm {
 };
 #endif
 
-static inline uint32_t esize(uint32_t st) { return st == ST_U8 ? 1u : (st == ST_U16 ? 2u : 4u); }
-
 } // namespace
 
 extern "C" void ojb_params_to_internal(const ojb_params* s, ojb::Params& P);     // ojb_capi.cpp (not part of the public header)
@@ -251,14 +249,14 @@ int ojb_shard_enc_configure(ojb_shard* s, const ojb_params* p, uint32_t sample_t
 
 // ---- row regions --------------------------------------------------------------------------------------------------
 // Encode: every rank uploads the image rows its slab's coefficients depend on (slab + halo), runs its window of every
-// DWT level and codes its own code-blocks (Encoder::PHASE_FRONT).  Then the one exchange of the path: each rank packs
+// DWT level and codes its own code-blocks (Encoder::encode_front).  Then the one exchange of the path: each rank packs
 // its blocks' bytes back to back behind the per-block lengths and sends them to the writer (sizes by one 8-byte
 // allgather), the writer drops them into its slot arena as if it had coded them (scatter_blocks_kernel) and finishes
-// as a single encoder does: packet headers, markers and layout on the device (Encoder::PHASE_BACK).  Byte-identical
+// as a single encoder does: packet headers, markers and layout on the device (Encoder::encode_back).  Byte-identical
 // to the one-GPU / reference codestream -- also for a single-tile image, which tile sharding cannot split.
 static void region_upload(ojb_shard* s, const void* const* planes, const uint32_t* strides) {
   Encoder& E = s->enc; const Params& P = E.params;
-  const uint32_t nc = P.num_comps(), es = esize(s->sample_type);
+  const uint32_t nc = P.num_comps(), es = esize_of(s->sample_type);
   for (const TileGeom& t : E.layout.tiles)
     for (uint32_t c = 0; c < nc; ++c) {
       const Rect& r = t.comps[c].rect;
@@ -282,9 +280,7 @@ static void region_encode(ojb_shard* s, const void* const* planes, const uint32_
   if (planes) region_upload(s, planes, strides);
   if (encode_only_upload) { cuda_check(cudaStreamSynchronize(E.stream), "region upload"); return; }
   // 1. this rank's share of the transform and of the block coding
-  E.phase = Encoder::PHASE_FRONT;
-  try { E.encode(nullptr, nullptr, false, nullptr, 0, true); } catch (...) { E.phase = Encoder::PHASE_ALL; throw; }
-  E.phase = Encoder::PHASE_ALL;
+  E.encode_front();
   cudaEventRecord(e1, E.stream);
   // 2. how many bytes that made; every rank learns every total
   s->d_off.reserve(((size_t)nb + 4) * 8);
@@ -325,9 +321,7 @@ static void region_encode(ojb_shard* s, const void* const* planes, const uint32_
     uint64_t sum = 0; for (uint32_t r = 0; r < C.world; ++r) sum += tot[r];
     const size_t cap = (size_t)sum + (size_t)nb * 24 + E.fixed_blob.size() + E.main_header.size() + (1u << 16);
     s->d_final.reserve(cap + 64);
-    E.phase = Encoder::PHASE_BACK;
-    try { total = E.encode(nullptr, nullptr, false, s->d_final.as<uint8_t>(), cap, true); } catch (...) { E.phase = Encoder::PHASE_ALL; throw; }
-    E.phase = Encoder::PHASE_ALL;
+    total = E.encode_back(s->d_final.as<uint8_t>(), cap);
     if (out) {
       if (total > out_cap) fail(0x000B0030, "output buffer too small: need %zu bytes, have %zu", total, (size_t)out_cap);
       cuda_check(cudaMemcpyAsync(out, s->d_final.p, total, cudaMemcpyDeviceToHost, E.stream), "codestream D2H");
@@ -348,7 +342,7 @@ static void region_decode(ojb_shard* s, uint32_t sample_type, uint32_t writer_ra
   D.decode(nullptr, nullptr, false);
   cudaEventRecord(e1, D.stream);
   const Params& P = D.params;
-  const uint32_t nc = P.num_comps(), es = esize(sample_type);
+  const uint32_t nc = P.num_comps(), es = esize_of(sample_type);
   // every rank's slab of every tile-component, packed tile after tile, component after component
   std::vector<size_t> roff(C.world + 1, 0);
   for (uint32_t r = 0; r < C.world; ++r) {
@@ -416,7 +410,7 @@ static int shard_encode(ojb_shard* s, const void* const* planes, const uint32_t*
     if (s->enc.region.on()) { region_encode(s, planes, strides, out, out_cap, out_len, encode_only_upload); return; }
     Encoder& E = s->enc; Comm& C = *s->comm;
     const Params& P = E.params;
-    const uint32_t nc = P.num_comps(), es = esize(s->sample_type);
+    const uint32_t nc = P.num_comps(), es = esize_of(s->sample_type);
     const uint32_t ntiles = (uint32_t)E.layout.tiles.size();
     cudaEvent_t e0 = E.ev[CodecBase::EV_MAX - 3], e1 = E.ev[CodecBase::EV_MAX - 2], e2 = E.ev[CodecBase::EV_MAX - 1];
     cudaEventRecord(e0, E.stream);
@@ -580,7 +574,7 @@ static int shard_decode(ojb_shard* s, const uint8_t* cs, bool cs_on_device, uint
     cudaEventRecord(e1, D.stream);
     // 4. tile samples to the writer: every tile packed (component after component, tight rows) in a staging buffer
     const Params& P = D.params;
-    const uint32_t nc = P.num_comps(), es = esize(sample_type);
+    const uint32_t nc = P.num_comps(), es = esize_of(sample_type);
     std::vector<size_t> toff(ntiles + 1, 0);
     for (uint32_t t = 0; t < ntiles; ++t) {
       size_t b = 0;
