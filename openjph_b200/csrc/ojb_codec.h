@@ -132,7 +132,7 @@ public:
   std::vector<std::vector<RowSpan>> region_rows;     // [tile][comp]: encoder: image rows this rank reads; decoder: rows it delivers
   static RowSpan region_slab(const Rect& tc, uint32_t g, uint32_t world);
   void plan_region(bool forward);
-  bool no_stream_dwt = false;          // force the general shared-memory DWT kernels (tests)
+  bool no_stream_dwt = getenv("OJB_NO_STREAM_DWT") != nullptr;     // force the general shared-memory DWT kernels (tests)
   bool no_fast_blocks = getenv("OJB_NO_FAST_BLOCKS") != nullptr;   // force the general block-coder kernels (tests, A/B)
 };
 

@@ -228,11 +228,20 @@ uint32_t Params::subband_index(uint32_t c, uint32_t res, uint32_t band) const {
 namespace {
 // Step sizes for a decomposition structure / kernel the reference has no tables for (it only decodes them): the
 // same recipe as set_rev_quant / set_irrev_quant (ojph_params.cpp:1495-1599) with the gains measured on the
-// kernel itself.  1-D, linearised (a reversible step is a / 2^e without rounding), symmetric extension, even origin:
+// kernel itself, 1-D and linearised (a reversible step is a / 2^e without rounding), for every level count a component
+// can have (DEPTH):
 //   bibo_l[n] / bibo_h[n]: worst-case amplification of n low-pass stages / of n - 1 low-pass stages and a high-pass one
 //   norm_l[n] / norm_h[n]: L2 norm of the synthesis waveform of one coefficient of those bands
+// Up to FINITE levels they are measured on a line of 16 << FINITE samples with symmetric extension, even origin (the
+// BIBO gains from the whole analysis matrix); the codestreams of such structures keep the steps they always had.
+// Deeper levels take the waveforms on an unbounded line: a unit impulse in the band carried back through n stages,
+// by synthesis or by the transpose of analysis (the transpose of the step "x[i] += a (x[i-1] + x[i+1]) on parity p"
+// is the same step on parity 1 - p, and the transposed stage runs the steps in synthesis order).  The work doubles
+// with every level, so past EXACT levels the gains continue at the ratio they settle to: the L2 norms at their last
+// measured ratio (sqrt(2) for the 9/7), the L1 norms at the DC gain of a low-pass analysis stage (one for every kernel
+// whose low-pass passes DC unchanged).
 struct KernelGains {
-  enum { DEPTH = 6 };
+  enum { DEPTH = 32, FINITE = 6, EXACT = 12 };
   double bibo_l[DEPTH + 1], bibo_h[DEPTH + 1], norm_l[DEPTH + 1], norm_h[DEPTH + 1];
   static double coef(const AtkSpec& k, size_t s) { return k.reversible() ? (double)k.steps[s].a / (double)(1u << k.steps[s].e) : (double)k.steps[s].A; }
   // one analysis stage on the first len entries of every column of m (rows = samples), even origin
@@ -269,19 +278,38 @@ struct KernelGains {
     }
     for (size_t i = 0; i < len; ++i) x[i] = t[i];
   }
+  // the waveform of one coefficient of the low (hi = false) or high band of stage n on an unbounded line, carried back
+  // to the input by synthesis or by the transposed analysis
+  static std::vector<double> waveform(const AtkSpec& k, int n, bool hi, bool analysis) {
+    const size_t N = k.steps.size(), P = 2 * (N / 2 + 1);      // even margin: every step widens the support by one
+    const double K = k.reversible() ? 1.0 : (double)k.K;
+    const double sl = analysis ? 1.0 / K : K, sh = analysis ? K : 1.0 / K;
+    std::vector<double> x(1, 1.0);
+    for (int j = n; j >= 1; --j) {
+      const bool high = hi && j == n;
+      std::vector<double> t(2 * x.size() + 2 * P, 0.0);
+      for (size_t i = 0; i < x.size(); ++i) t[P + 2 * i + (high ? 1 : 0)] = x[i] * (high ? sh : sl);
+      for (size_t s = 0; s < N; ++s) {
+        const double a = analysis ? coef(k, s) : -coef(k, s);
+        for (size_t i = 2 - ((s & 1) ^ (analysis ? 1 : 0)); i + 1 < t.size(); i += 2) t[i] += a * (t[i - 1] + t[i + 1]);
+      }
+      x.swap(t);
+    }
+    return x;
+  }
   explicit KernelGains(const AtkSpec& k) {
-    const size_t L = (size_t)16 << DEPTH;
+    const size_t L = (size_t)16 << FINITE;
     bibo_l[0] = norm_l[0] = 1.0; bibo_h[0] = norm_h[0] = 1.0;
     std::vector<std::vector<double>> m(L, std::vector<double>(L, 0.0));
     for (size_t i = 0; i < L; ++i) m[i][i] = 1.0;
     size_t len = L;
     auto worst = [&](size_t a, size_t b) { double g = 0; for (size_t i = a; i < b; ++i) { double s = 0; for (double v : m[i]) s += std::fabs(v); g = std::max(g, s); } return g; };
-    for (int n = 1; n <= DEPTH; ++n) {
+    for (int n = 1; n <= FINITE; ++n) {
       analyse(m, len, k);
       bibo_l[n] = worst(0, len / 2); bibo_h[n] = worst(len / 2, len);
       len /= 2;
     }
-    for (int n = 1; n <= DEPTH; ++n) {
+    for (int n = 1; n <= FINITE; ++n) {
       for (int hi = 0; hi < 2; ++hi) {
         std::vector<double> x(L, 0.0);
         size_t l = L >> n;                         // length of the low band after n stages
@@ -291,8 +319,23 @@ struct KernelGains {
         (hi ? norm_h : norm_l)[n] = std::sqrt(e);
       }
     }
+    for (int n = FINITE + 1; n <= EXACT; ++n) {
+      for (int hi = 0; hi < 2; ++hi) {
+        double l1 = 0, l2 = 0;
+        for (double v : waveform(k, n, hi != 0, true)) l1 += std::fabs(v);
+        for (double v : waveform(k, n, hi != 0, false)) l2 += v * v;
+        (hi ? bibo_h : bibo_l)[n] = l1;
+        (hi ? norm_h : norm_l)[n] = std::sqrt(l2);
+      }
+    }
+    double dc = 0;
+    for (double v : waveform(k, 1, false, true)) dc += v;
+    const double rl = norm_l[EXACT] / norm_l[EXACT - 1], rh = norm_h[EXACT] / norm_h[EXACT - 1];
+    for (int n = EXACT + 1; n <= DEPTH; ++n) {
+      bibo_l[n] = bibo_l[n - 1] * std::fabs(dc); bibo_h[n] = bibo_h[n - 1] * std::fabs(dc);
+      norm_l[n] = norm_l[n - 1] * rl; norm_h[n] = norm_h[n - 1] * rh;
+    }
   }
-  static int clampd(uint32_t n) { return (int)std::min<uint32_t>(n, DEPTH); }
 };
 } // namespace
 
@@ -375,15 +418,14 @@ std::vector<Part2Band> part2_bands(uint32_t comp, const Params& p) {
     return n;
   };
   {
-    int nx = KernelGains::clampd(count(D, true)), ny = KernelGains::clampd(count(D, false));
+    const uint32_t nx = count(D, true), ny = count(D, false);
     bands.push_back(B{ g.bibo_l[nx] * g.bibo_l[ny], g.norm_l[nx] * g.norm_l[ny], 0 });
   }
   for (uint32_t r = 1; r <= D; ++r) {
     const uint32_t level = D - r + 1;
     const DfsType t = p.dwt_type(comp, level);
     const bool hx = t == DFS_BIDIR || t == DFS_HORZ, vy = t == DFS_BIDIR || t == DFS_VERT;
-    const int nx = KernelGains::clampd(count(level - 1, true)), ny = KernelGains::clampd(count(level - 1, false));
-    const int nx1 = KernelGains::clampd((uint32_t)nx + 1), ny1 = KernelGains::clampd((uint32_t)ny + 1);
+    const uint32_t nx = count(level - 1, true), ny = count(level - 1, false), nx1 = nx + 1, ny1 = ny + 1;
     for (uint32_t b = 1; b < 4; ++b) {
       const bool bh = (b & 1) != 0, bv = (b & 2) != 0;
       if ((bh && !hx) || (bv && !vy)) continue;

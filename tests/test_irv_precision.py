@@ -86,7 +86,10 @@ BIG_CASES = [
 ALL = dict(CPU_CASES + BIG_CASES)
 # the variant runs (switches read once per process) take this subset
 VARIANT_CASES = ["w121_x1", "w241_x1", "ict_u16_12bit", "levels5_deep", "thin_3x6", "fine_qstep_kmax16", "q90_split"]
-VARIANTS = {"no_fast_blocks": {"OJB_NO_FAST_BLOCKS": "1"}}
+# no_stream_dwt: every level through the general shared-memory kernels (dwt_fwd.cu / dwt_inv.cu), which otherwise only
+# take dyadic 9/7 levels of frames whose coefficients pass 2^30 words; on the GPU with a 4K frame as well
+VARIANTS = {"no_fast_blocks": {"OJB_NO_FAST_BLOCKS": "1"}, "no_stream_dwt": {"OJB_NO_STREAM_DWT": "1"}}
+VARIANT_GPU_EXTRA = {"no_stream_dwt": ["cfg5_3840x2160_10bit"]}
 
 
 # ---- the streaming DWT's tiling (dwt_stream_tiling, dwt_stream.cu), restated to choose and audit the sizes -------
@@ -375,7 +378,8 @@ def _variant_child(variant, gpu):
         pytest.skip("already inside the child run")
     env = dict(os.environ, OJB_IRV_VARIANT_CHILD="1", **VARIANTS[variant])
     args = [sys.executable, "-m", "pytest", os.path.abspath(__file__), "-x", "-q", "-p", "no:cacheprovider",
-            "-k", ("gpu and (%s)" if gpu else "emulated and (%s)") % " or ".join(VARIANT_CASES)]
+            "-k", ("gpu and (%s)" if gpu else "emulated and (%s)") % " or ".join(
+                VARIANT_CASES + (VARIANT_GPU_EXTRA.get(variant, []) if gpu else []))]
     if gpu:
         args += ["-m", "gpu"]
     r = subprocess.run(args, env=env, capture_output=True, text=True, cwd=ROOT)
