@@ -295,11 +295,35 @@ int ojb_enc_quality_info(ojb_encoder* e, ojb_quality_info* out);
  * both); 0x000B0050 a configuration on the 64-bit coefficient path (no target size or quality there); 0x000B0051 a
  * truncated or damaged codestream, or a code-block that fails to decode (there is no resilient transcode);
  * 0x000B0052 ojb_enc_transcode before ojb_enc_transcode_headers; 0x000B0053 a pixel frame call (encode, upload, raster,
- * lines) on an encoder configured by ojb_enc_transcode_headers.  A refused input leaves the encoder as it was. */
+ * lines) on an encoder configured by ojb_enc_transcode_headers.  A refused input leaves the encoder as it was.
+ *
+ * Reduced resolution (ojb_enc_transcode_headers_reduced, skipped_res = r > 0): the output is the input with its top r
+ * resolution levels dropped, as ojph_expand -skip_res r would reconstruct it -- a 2K stream from a 4K master, a proxy or
+ * a thumbnail stream -- from the kept code-blocks alone.  SIZ's extent, image offset and tile offset become
+ * ceil(v / 2^r), and the tile size XTsiz / 2^r along a direction with more than one tile; so every kept tile, resolution,
+ * band, precinct and code-block keeps its rectangle.  COD and every COC lose r levels (and their precinct sizes of the
+ * dropped resolutions), QCD and every QCC keep their first 1 + 3 (D_c - r) step sizes (guard bits and Sqcd as they
+ * are), CAP's MAGB is recomputed, and every other main-header segment is copied.  The tile-part division kind and the
+ * TLM follow the input's.  Without a target every kept block is re-coded as the input carried it, and the reference
+ * decoder's output of the result equals its decode of the input restricted to (r, r), sample for sample; a quality
+ * target's source is that restricted decode.  ojb_enc_transcode, the target setters, ojb_enc_min_size,
+ * ojb_enc_rate_info and ojb_enc_quality_info describe the output geometry.  r = 0 is ojb_enc_transcode_headers.
+ * Errors besides the ones above: 0x000300A2 r above COD's level count, 0x000B0007 r above a component's own (COC) count
+ * (both as ojb_dec_restrict_input_resolution; r equal to a count leaves that component without levels, which is
+ * valid); 0x000B0054 a DFS decomposition structure (a dropped level's split would set the reduction per direction and
+ * renumber the step sizes; ATK kernels alone are fine); 0x000B0055 a tile grid that does not survive the reduction
+ * (several tiles along a direction whose tile size is not a multiple of 2^r, or a tile that would keep no samples:
+ * tile indices, tile-parts and TLM entries stay one-to-one with the input's); 0x000B0056 the input's Rsiz names the
+ * broadcast or IMF profile (bits 8-11, without the Part 2 flag) and the reduced parameters break that profile's rules
+ * (e.g. broadcast needs 1 to 5 levels). */
 /* the encoder counterpart of ojb_dec_read_headers: configures e from a codestream's headers and tile-parts (host
  * memory, or device memory when on_device, with >= 32 readable bytes after its end); the target setters follow it as
  * they follow ojb_enc_configure */
 int ojb_enc_transcode_headers(ojb_encoder* e, const void* j2c, uint64_t len, int on_device, uint32_t sample_type);
+/* the same for an output with the input's top skipped_res resolution levels dropped; info (may be null) receives the
+ * output's geometry, as a decoder of the output reports it */
+int ojb_enc_transcode_headers_reduced(ojb_encoder* e, const void* j2c, uint64_t len, int on_device, uint32_t sample_type,
+                                      uint32_t skipped_res, ojb_frame_info* info);
 /* re-codes the codestream (same main header and tile-part structure as the headers call, else it is read again) to
  * e's target; out on the device when out_on_device */
 int ojb_enc_transcode(ojb_encoder* e, const void* j2c, uint64_t len, int on_device,

@@ -130,6 +130,7 @@ SYMBOLS = {
     "ojb_enc_min_size": (_I, [_VP, C.POINTER(_U64)]),
     "ojb_enc_set_target_mse": (_I, [_VP, C.c_double]),
     "ojb_enc_transcode_headers": (_I, [_VP, _VP, _U64, _I, _U32]),
+    "ojb_enc_transcode_headers_reduced": (_I, [_VP, _VP, _U64, _I, _U32, _U32, C.POINTER(FrameInfo)]),
     "ojb_enc_transcode": (_I, [_VP, _VP, _U64, _I, _VP, _U64, C.POINTER(_U64), _I]),
     "ojb_enc_quality_info": (_I, [_VP, C.POINTER(QualityInfo)]),
     "ojb_enc_rate_info": (_I, [_VP, C.POINTER(_U32), C.POINTER(_U32), _VP, _VP, _VP, _VP, C.POINTER(_U64), C.POINTER(C.c_float)]),

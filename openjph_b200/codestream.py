@@ -237,12 +237,17 @@ class Encoder(_Base):
         self.set_target_mse(peak * peak / 10.0 ** (float(db) / 10.0))
 
     @classmethod
-    def from_codestream(cls, j2c, sample_type=I32, target_bytes=None, target_mse=None, target_psnr=None, lib=None):
+    def from_codestream(cls, j2c, sample_type=I32, target_bytes=None, target_mse=None, target_psnr=None, lib=None,
+                        skipped_res=0):
         """an encoder configured from a codestream's headers and tile-parts (bytes or a uint8 array in host memory, or
         a 1-D CUDA uint8 tensor), which transcodes: transcode() re-codes such a codestream from its code-blocks,
         single-layer and cleanup-only, with the input's geometry, coding parameters, main header (less TLM / PLM) and
         tile-parts, to the targets given here or set later.  The source of a quality target is the input as the
-        Decoder returns it in `sample_type`; target_psnr takes the bit depth from the headers."""
+        Decoder returns it in `sample_type`; target_psnr takes the bit depth from the headers.
+
+        skipped_res=r > 0 drops the input's top r resolution levels (as ojph_expand -skip_res r): the output is the
+        reduced-resolution codestream the kept code-blocks make, whose decode equals the input's decode restricted to
+        (r, r), and a quality target's source is that restricted decode.  `dims` are the output's component sizes."""
         self = cls.__new__(cls)
         _Base.__init__(self, lib)
         self.h = self.L.ojb_enc_create()
@@ -251,8 +256,15 @@ class Encoder(_Base):
         self.params = None
         self.sample_type = sample_type
         ptr, n, dev, head = self._codestream(j2c)
-        self._check(self.L.ojb_enc_transcode_headers(self.h, ptr, n, dev, sample_type))
-        self.dims, self._depths = _siz_of(head)
+        if skipped_res == 0:
+            self._check(self.L.ojb_enc_transcode_headers(self.h, ptr, n, dev, sample_type))
+            self.dims, self._depths = _siz_of(head)
+        else:
+            info = _lib.FrameInfo()
+            self._check(self.L.ojb_enc_transcode_headers_reduced(self.h, ptr, n, dev, sample_type, int(skipped_res),
+                                                                 C.byref(info)))
+            self.dims = [(int(info.comp_w[c]), int(info.comp_h[c])) for c in range(info.num_comps)]
+            self._depths = [int(info.bit_depth[c]) for c in range(info.num_comps)]
         self._out = np.empty(sum(w * h for w, h in self.dims) * 4 + (1 << 20), np.uint8)
         if target_bytes:
             self.set_target_size(target_bytes)

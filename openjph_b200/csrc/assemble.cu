@@ -151,14 +151,16 @@ dec_merge_kernel(DecBlock* __restrict__ blocks, const DecBlock* __restrict__ pro
 
 // the transcoder's block array of one frame: block b as the encoder configured it, started at the lowest plane q_b the
 // input codes it down to (the decoder's gates: SigProp / MagRef passes count only with bytes and with p > 1); a block the
-// input leaves out gets p = 31, which leaves it zero candidates
+// input leaves out gets p = 31, which leaves it zero candidates.  map (null: the identity) names the input's block
+// behind each of the encoder's when the output drops resolution levels
 __global__ void __launch_bounds__(256)
-transcode_blocks_kernel(const EncBlock* __restrict__ geom, const DecBlock* __restrict__ dec, uint32_t n, EncBlock* __restrict__ out)
+transcode_blocks_kernel(const EncBlock* __restrict__ geom, const DecBlock* __restrict__ dec, const uint32_t* __restrict__ map,
+                        uint32_t n, EncBlock* __restrict__ out)
 {
   const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= n) return;
   EncBlock e = geom[b];
-  const DecBlock d = dec[b];
+  const DecBlock d = dec[map ? map[b] : b];
   const bool refined = d.num_passes > 1 && d.len2 != 0 && d.missing_msbs < 29;
   if (d.num_passes == 0 || d.len1 == 0) { e.p = 31; e.flags &= (uint16_t)~ENC_CHECK_NEGZERO; }
   else e.p = (uint16_t)((refined ? 29u : 30u) - d.missing_msbs);
@@ -173,10 +175,11 @@ void launch_dec_merge(DecBlock* blocks, const DecBlock* proto, const DecDyn* dyn
   OJB_LAUNCH(dec_merge_kernel, dim3((nblocks + 255) / 256), dim3(256), 0, st, blocks, proto, dyn, nblocks);
 }
 
-void launch_transcode_blocks(const EncBlock* geom, const DecBlock* dec, uint32_t nblocks, EncBlock* out, cudaStream_t st)
+void launch_transcode_blocks(const EncBlock* geom, const DecBlock* dec, const uint32_t* map, uint32_t nblocks, EncBlock* out,
+                             cudaStream_t st)
 {
   if (nblocks == 0) return;
-  OJB_LAUNCH(transcode_blocks_kernel, dim3((nblocks + 255) / 256), dim3(256), 0, st, geom, dec, nblocks, out);
+  OJB_LAUNCH(transcode_blocks_kernel, dim3((nblocks + 255) / 256), dim3(256), 0, st, geom, dec, map, nblocks, out);
 }
 
 void launch_ctrl_copy(void* dst, const void* src, size_t bytes, cudaStream_t st)

@@ -440,13 +440,35 @@ int ojb_enc_rate_info(ojb_encoder* e, uint32_t* num_blocks, uint32_t* kc, uint8_
     if (ms4) for (int i = 0; i < 4; ++i) ms4[i] = E.rc_ms[i];
   });
 }
-int ojb_enc_transcode_headers(ojb_encoder* e, const void* j2c, uint64_t len, int on_device, uint32_t sample_type) {
+int ojb_enc_transcode_headers_reduced(ojb_encoder* e, const void* j2c, uint64_t len, int on_device, uint32_t sample_type,
+                                      uint32_t skipped_res, ojb_frame_info* info) {
   return guarded_on(e->device, [&] {
     if (sample_type > 2) fail(0x000B0012, "unknown sample container");
     e->configured = false;               // a failing call leaves no half-built encoder behind
-    e->enc.transcode_headers(static_cast<const uint8_t*>(j2c), (size_t)len, on_device != 0, sample_type);
+    e->enc.transcode_headers(static_cast<const uint8_t*>(j2c), (size_t)len, on_device != 0, sample_type, skipped_res);
     e->configured = true;
+    if (info) {
+      // the output's geometry: what a decoder of the transcoded stream reports
+      const Params& P = e->enc.params;
+      FrameInfo fi; memset(&fi, 0, sizeof(fi));
+      fi.width = P.Xsiz; fi.height = P.Ysiz; fi.off_x = P.XOsiz; fi.off_y = P.YOsiz;
+      fi.num_comps = P.num_comps();
+      for (uint32_t c = 0; c < fi.num_comps && c < 16; ++c) {
+        fi.bit_depth[c] = P.comps[c].bit_depth; fi.is_signed[c] = P.comps[c].is_signed;
+        fi.dx[c] = P.comps[c].dx; fi.dy[c] = P.comps[c].dy;
+        fi.comp_w[c] = P.comp_width(c); fi.comp_h[c] = P.comp_height(c);
+        fi.nlt_type[c] = P.nlt_type(c);
+      }
+      fi.num_decomps = P.num_decomps; fi.reversible = P.reversible();
+      fi.color_transform = P.color_transform();
+      fi.num_tiles = (uint32_t)e->enc.layout.tiles.size();
+      static_assert(sizeof(FrameInfo) == sizeof(ojb_frame_info), "frame info layout");
+      memcpy(info, &fi, sizeof(fi));
+    }
   });
+}
+int ojb_enc_transcode_headers(ojb_encoder* e, const void* j2c, uint64_t len, int on_device, uint32_t sample_type) {
+  return ojb_enc_transcode_headers_reduced(e, j2c, len, on_device, sample_type, 0, nullptr);
 }
 int ojb_enc_transcode(ojb_encoder* e, const void* j2c, uint64_t len, int on_device,
                       uint8_t* out, uint64_t out_cap, uint64_t* out_len, int out_on_device) {

@@ -1583,7 +1583,7 @@ BlockFrame Decoder::frame_records(uint32_t dec_out, DecDyn* hy) {
 void Decoder::enqueue_blocks(const BlockFrame& f, const DecDyn* hy, const uint8_t* cs, uint32_t* coef, cudaStream_t st,
                              const SideStream* sd, uint32_t& launches) {
   const uint32_t nb = (uint32_t)h_dec_proto.size();
-  if (nb) { launch_dec_merge(d_dec.as<DecBlock>(), d_proto.as<DecBlock>(), hy, nb, st); ++launches; }
+  if (nb) { launch_dec_merge(d_dec.as<DecBlock>(), out_proto ? out_proto : d_proto.as<DecBlock>(), hy, nb, st); ++launches; }
   if (wide) {
     if (!f.cleanup_only) fail(0x000B0009, "SigProp / MagRef passes are not implemented on the 64-bit coefficient path");
     launch_ht_decode_wide(d_dec.as<DecBlock>(), nb, max_block_w, cs, coef, d_tables_dec.as<uint16_t>(), false,
@@ -1687,12 +1687,16 @@ namespace ojb {
 // Transcoder (see ojb_codec.h)
 //------------------------------------------------------------------------------------------
 // The input's parse, what it refuses and the configuration it implies: the input's coding parameters, its main header
-// without TLM / PLM, its tile-part division and whether it had a TLM.  The encoder is configured again only when that
-// changed, and only after every check passed, so a refused input leaves the encoder as it was.
-void Encoder::transcode_parse(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type) {
+// without TLM / PLM, its tile-part division and whether it had a TLM -- or, with skipped_res = r > 0, the parameters and
+// main header of the input with its top r resolution levels dropped (reduce_main_header), with the same tile-part
+// division kind and TLM.  The encoder is configured again only when that changed, and only after every check passed,
+// so a refused input leaves the encoder as it was.
+void Encoder::transcode_parse(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type, uint32_t skipped_res) {
   if (!src) { src.reset(new Decoder()); src->parse_only = true; }
   Decoder& D = *src;
   if (on_device) D.read_headers_device(j2c, len, sample_type); else D.read_headers(j2c, len, sample_type);
+  // the dropped resolutions' blocks are skipped (Decoder::frame_records); restrict_resolution would also plan an image
+  D.skip_read = D.skip_recon = skipped_res;
   if (D.params.uses_sop() || D.params.uses_eph())
     fail(0x000B004C, "the codestream uses SOP or EPH markers (Scod bits 1-2), which a transcode does not write");
   if (D.wide)
@@ -1737,19 +1741,77 @@ void Encoder::transcode_parse(const uint8_t* j2c, size_t len, bool on_device, ui
   if (div < 0)
     fail(0x000B004F, "the codestream's tile-parts follow none of the divisions a transcode writes (none, by resolution, by "
          "component, by both)");
-  if (transcoding && hdr == main_header && params.tilepart_div == (uint32_t)div && params.need_tlm == tlm && img_type == sample_type)
+  if (transcoding && hdr == xc_in_header && xc_skip == skipped_res && params.tilepart_div == (uint32_t)div &&
+      params.need_tlm == tlm && img_type == sample_type)
     return;
+  Params np;
+  std::vector<uint8_t> out_hdr;
+  if (skipped_res) {
+    reduce_main_header(hdr, D.params, skipped_res, out_hdr, np);
+    np.planar = np.color_transform() ? 0 : 1;       // as the decoder derives it (Decoder::read_headers)
+  } else {
+    np = D.params;
+    out_hdr = hdr;
+  }
   transcoding = false;                  // a failing setup leaves no half-configured transcoder
-  params = D.params;
+  D.out_proto = nullptr;
+  params = np;
   params.tilepart_div = (uint32_t)div; params.need_tlm = tlm;
-  main_header.swap(hdr);
+  main_header.swap(out_hdr);
+  xc_in_header.swap(hdr);
+  xc_skip = skipped_res;
   transcoding = true;
-  try { setup(sample_type); } catch (...) { transcoding = false; throw; }
+  try { setup(sample_type); plan_block_map(); } catch (...) { transcoding = false; throw; }
 }
 
-void Encoder::transcode_headers(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type) {
+// The block correspondence of a transcode that drops resolution levels.  The input's blocks of resolution k <= D_c - r
+// are the output's blocks of resolution k, band for band, with the same rectangles (reduce_main_header).  But the
+// restricted decoder's arena does not match the encoder's: Layout::build lays each tile-component out from its finest
+// resolution down, so the dropped resolutions' planes come first and push every kept plane to another offset, and the
+// block numbers (band by band in the same order) shift the same way.  So each kept block's prototype gets the
+// encoder's plane offset and stride, and the encoder's block b reads the decoder's record map[b].
+void Encoder::plan_block_map() {
+  Decoder& D = *src;
+  D.out_proto = nullptr;
+  if (xc_skip == 0) return;
+  std::vector<uint32_t> map(layout.num_blocks, 0);
+  std::vector<DecBlock> proto(D.h_dec_proto);
+  auto same = [](const Rect& a, const Rect& b) { return a.x0 == b.x0 && a.y0 == b.y0 && a.w == b.w && a.h == b.h; };
+  for (size_t t = 0; t < layout.tiles.size(); ++t)
+    for (size_t c = 0; c < layout.tiles[t].comps.size(); ++c) {
+      const TileCompGeom& ec = layout.tiles[t].comps[c];
+      const TileCompGeom& dc = D.layout.tiles[t].comps[c];
+      if (ec.res.size() + xc_skip != dc.res.size() || !same(ec.rect, dc.res[ec.res.size() - 1].rect))
+        fail(0x000B0051, "internal: tile %zu component %zu of the reduced geometry is not the input's", t, c);
+      for (size_t k = 0; k < ec.res.size(); ++k)
+        for (uint32_t b = 0; b < 4; ++b) {
+          const BandGeom& eb = ec.res[k].bands[b];
+          const BandGeom& db = dc.res[k].bands[b];
+          if (eb.empty != db.empty || (!eb.empty && (!same(eb.rect, db.rect) || eb.nbw != db.nbw || eb.nbh != db.nbh ||
+                                                      eb.xcb != db.xcb || eb.ycb != db.ycb || eb.K_max != db.K_max)))
+            fail(0x000B0051, "internal: band %u of resolution %zu of the reduced geometry is not the input's", b, k);
+          if (eb.empty) continue;
+          for (uint32_t by = 0; by < eb.nbh; ++by)
+            for (uint32_t bx = 0; bx < eb.nbw; ++bx) {
+              const uint32_t i = by * eb.nbw + bx;
+              const Rect r = eb.block_rect(bx, by);
+              DecBlock& p = proto[db.block_base + i];
+              map[eb.block_base + i] = db.block_base + i;
+              p.dst_off = eb.plane_off + eb.plane_pad_x + (uint64_t)(r.y0 - eb.rect.y0) * eb.plane_stride + (r.x0 - eb.rect.x0);
+              p.stride = eb.plane_stride;
+            }
+        }
+    }
+  d_xmap.reserve(std::max<size_t>(1, map.size()) * 4);
+  d_xproto.reserve(std::max<size_t>(1, proto.size()) * sizeof(DecBlock));
+  if (!map.empty()) CK(cudaMemcpy(d_xmap.p, map.data(), map.size() * 4, cudaMemcpyHostToDevice));
+  if (!proto.empty()) CK(cudaMemcpy(d_xproto.p, proto.data(), proto.size() * sizeof(DecBlock), cudaMemcpyHostToDevice));
+  D.out_proto = d_xproto.as<DecBlock>();
+}
+
+void Encoder::transcode_headers(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type, uint32_t skipped_res) {
   transcoding = false;
-  transcode_parse(j2c, len, on_device, sample_type);
+  transcode_parse(j2c, len, on_device, sample_type, skipped_res);
 }
 
 // the transform's place in the frame: the input to the device, [the source of a quality target: the input decoded as
@@ -1768,7 +1830,8 @@ void Encoder::enqueue_transcode_front() {
   }
   D.enqueue_blocks(xc_coded, D.h_dyn.as<DecDyn>(), xc_cs, d_coef.as<uint32_t>(), stream, &side, last_launches);
   if (nb) { launch_ctrl_copy(D.h_bstatus.p, D.d_bstatus.p, (size_t)nb * 4, stream); ++last_launches; }
-  launch_transcode_blocks(d_blocks.as<EncBlock>(), D.d_dec.as<DecBlock>(), nb, d_xblocks.as<EncBlock>(), stream);
+  launch_transcode_blocks(d_blocks.as<EncBlock>(), D.d_dec.as<DecBlock>(), xc_skip ? d_xmap.as<uint32_t>() : nullptr,
+                          (uint32_t)h_blocks.size(), d_xblocks.as<EncBlock>(), stream);
   ++last_launches;
 }
 
@@ -1776,7 +1839,7 @@ size_t Encoder::transcode(const uint8_t* j2c, size_t len, bool on_device, uint8_
   if (!transcoding)
     fail(0x000B0052, "a transcode needs ojb_enc_transcode_headers first: this encoder is not configured from a codestream");
   const auto t0 = std::chrono::steady_clock::now();
-  transcode_parse(j2c, len, on_device, img_type);
+  transcode_parse(j2c, len, on_device, img_type, xc_skip);
   Decoder& D = *src;
   const uint32_t nb = (uint32_t)D.h_dec_proto.size();
   DecDyn* hy = D.h_dyn.as<DecDyn>();

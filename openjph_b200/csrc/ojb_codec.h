@@ -267,10 +267,17 @@ public:
   // frame re-coded from that codestream's code-blocks (transcode), single-layer and cleanup-only, to the encoder's
   // target.  A parse-only decoder (no arena, image or synthesis jobs of its own) reads the input; its block decoders
   // write the coded sign-magnitude words (DEC_OUT_CODED) into d_coef, whose band planes sit where the decoder's do
-  // (one Layout of one parameter set).  d_xblocks is the frame's block array: block b at p = q_b, the lowest plane the
-  // input codes it down to (31: left out), so candidate k = 0 re-codes exactly the input's bits; rate control and the
-  // block coder read it in place of d_blocks.  With a quality target the source is the input decoded as the decoder
-  // would, into d_rcoef and through rq_jobs into d_image, which exists only then.
+  // when the output keeps the input's geometry (one Layout of one parameter set).  d_xblocks is the frame's block
+  // array: block b at p = q_b, the lowest plane the input codes it down to (31: left out), so candidate k = 0 re-codes
+  // exactly the input's bits; rate control and the block coder read it in place of d_blocks.  With a quality target the
+  // source is the input decoded as the decoder would, into d_rcoef and through rq_jobs into d_image, which exists only
+  // then.
+  //
+  // With xc_skip = r > 0 the output is the input with its top r resolution levels dropped (reduce_main_header derives
+  // its main header and parameters).  The parse-only decoder then reads the input restricted to (r, r): the dropped
+  // resolutions' blocks are marked skip and neither uploaded nor decoded.  The two sides number their blocks and lay out
+  // their arenas differently (see plan_block_map): d_xmap gives the input's block behind each of the encoder's, and
+  // d_xproto holds the input's block prototypes with each kept block's words sent to the encoder's band planes.
   std::unique_ptr<Decoder> src;
   bool transcoding = false;
   bool xc_two_pass = false;            // the frame has SigProp-without-MagRef blocks: k = 0 is not the source
@@ -278,9 +285,13 @@ public:
   PinnedBuf h_xdyn;                    // the source decode's block records (the coded decode's sit in src->h_dyn)
   const uint8_t* xc_cs = nullptr;      // the input on the device
   BlockFrame xc_coded, xc_source;      // the frame's two block decodes (the source: with a quality target only)
-  void transcode_headers(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type);
+  uint32_t xc_skip = 0;                // resolution levels the output drops
+  std::vector<uint8_t> xc_in_header;   // the input's main header (less TLM / PLM) this configuration was derived from
+  DeviceBuf d_xmap, d_xproto;          // xc_skip > 0 only
+  void transcode_headers(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type, uint32_t skipped_res = 0);
   size_t transcode(const uint8_t* j2c, size_t len, bool on_device, uint8_t* out, size_t out_cap, bool out_on_device);
-  void transcode_parse(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type);
+  void transcode_parse(const uint8_t* j2c, size_t len, bool on_device, uint32_t sample_type, uint32_t skipped_res);
+  void plan_block_map();
   void enqueue_transcode_front();
 };
 
@@ -344,6 +355,8 @@ public:
   // jobs or refinement scratch (enqueue_blocks reserves the scratch when a frame has refinement passes)
   bool parse_only = false;
   size_t scratch_words = 0;
+  // the transcoder's block prototypes when its output lays out the kept blocks elsewhere (null: d_proto)
+  const DecBlock* out_proto = nullptr;
   // the block records of the parsed frame into hy, for the output mode dec_out; the block decoders of those records
   // into the arena coef on stream st (launches counted)
   BlockFrame frame_records(uint32_t dec_out, DecDyn* hy);

@@ -32,8 +32,9 @@ void launch_ht_decode_serial(const DecBlock* blocks, uint32_t nblocks, uint32_t 
 // dyn may be mapped pinned host memory (read by the SMs, like launch_ctrl_copy)
 void launch_dec_merge(DecBlock* blocks, const DecBlock* proto, const DecDyn* dyn, uint32_t nblocks, cudaStream_t st);
 // transcoding: out[b] = geom[b] (the encoder's static block array) with p = q_b, the lowest plane the merged decoder
-// record dec[b] codes (31: the block is left out)
-void launch_transcode_blocks(const EncBlock* geom, const DecBlock* dec, uint32_t nblocks, EncBlock* out, cudaStream_t st);
+// record dec[map[b]] codes (31: the block is left out); map null: the identity
+void launch_transcode_blocks(const EncBlock* geom, const DecBlock* dec, const uint32_t* map, uint32_t nblocks, EncBlock* out,
+                             cudaStream_t st);
 
 // 64-bit samples (precision beyond 32 bits): cleanup pass only, output int64 (or the raw sign-magnitude words)
 void launch_ht_decode_wide(const DecBlock* blocks, uint32_t nblocks, uint32_t max_width, const uint8_t* codestream,

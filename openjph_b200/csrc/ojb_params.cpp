@@ -3,6 +3,7 @@
 #include <cmath>
 #include <cstring>
 #include <algorithm>
+#include <algorithm>
 
 namespace ojb {
 
@@ -515,6 +516,25 @@ static void make_quant_steps(QuantSet& q, uint32_t comp, const Params& p) {
   }
 }
 
+uint32_t Params::cap_magb() const {
+  // MAGB over QCD and every QCC (ojph_params.cpp:1615)
+  uint32_t B = 0;
+  const bool part2 = any_part2();
+  auto magb = [&](const QuantSet& q) {
+    uint32_t nd = (q.num_subbands - 1) / 3;
+    for (uint32_t i = 0; i < q.num_subbands; ++i) {
+      uint32_t t;
+      if (part2) { B = std::max(B, q.kmax_at(i)); continue; }      // no dyadic level to take the band's gain from
+      if ((q.Sqcd & 0x1F) == 0) t = ((uint32_t)(q.SP[i] & 0xFF) >> 3) + q.guard_bits() - 1u;
+      else { uint32_t nb = nd - (i ? (i - 1) / 3 : 0); t = (uint32_t)(q.SP[i] >> 11) + q.guard_bits() - nb; }
+      B = std::max(B, t);
+    }
+  };
+  magb(qcd);
+  for (const QuantSet& q : qcc) magb(q);
+  return (B <= 8) ? 0 : (B < 28 ? B - 8 : 13 + (B >> 2));
+}
+
 void Params::finalize_for_encode() {
   // tile size 0x0 => one tile covering the image (ojph_codestream_local.cpp:562-570)
   if (XTsiz == 0 && YTsiz == 0) { XTsiz = Xsiz + XOsiz; YTsiz = Ysiz + YOsiz; }
@@ -620,25 +640,10 @@ void Params::finalize_for_encode() {
     make_quant_steps(*q, c, *this);
   }
 
-  // CAP (ojph_params_local.h:982-998); MAGB over QCD and every QCC (ojph_params.cpp:1615)
+  // CAP (ojph_params_local.h:982-998)
   if (reversible()) Ccap0 &= 0xFFDF; else Ccap0 |= 0x0020;
   Ccap0 &= 0xFFE0;
-  uint32_t B = 0;
-  const bool part2 = any_part2();
-  auto magb = [&](const QuantSet& q) {
-    uint32_t nd = (q.num_subbands - 1) / 3;
-    for (uint32_t i = 0; i < q.num_subbands; ++i) {
-      uint32_t t;
-      if (part2) { B = std::max(B, q.kmax_at(i)); continue; }      // no dyadic level to take the band's gain from
-      if ((q.Sqcd & 0x1F) == 0) t = ((uint32_t)(q.SP[i] & 0xFF) >> 3) + q.guard_bits() - 1u;
-      else { uint32_t nb = nd - (i ? (i - 1) / 3 : 0); t = (uint32_t)(q.SP[i] >> 11) + q.guard_bits() - nb; }
-      B = std::max(B, t);
-    }
-  };
-  magb(qcd);
-  for (const QuantSet& q : qcc) magb(q);
-  uint32_t Bp = (B <= 8) ? 0 : (B < 28 ? B - 8 : 13 + (B >> 2));
-  Ccap0 = (uint16_t)(Ccap0 | (uint16_t)Bp);
+  Ccap0 = (uint16_t)(Ccap0 | (uint16_t)cap_magb());
 
   (void)needs_wide();        // 64-bit coefficients: reversible components only (refuses the rest)
 
@@ -1165,6 +1170,116 @@ size_t Params::read_main_header(const uint8_t* data, size_t len) {
     }
   if (received != 3) fail(0x00030052, "markers error, COD and QCD are required");
   return r.pos;
+}
+
+//------------------------------------------------------------------------------------------
+// The same codestream with its top resolution levels dropped
+//------------------------------------------------------------------------------------------
+// The profile a codestream's Rsiz names in its Part 1 field (bits 8-11, meaningful only without the Part 2 flag,
+// bit 15): 1-3 broadcast, 4-9 IMF.  Returned as Params::profile (0 none, 1 IMF, 2 broadcast).
+static uint32_t claimed_profile(uint16_t Rsiz) {
+  if (Rsiz & 0x8000) return 0;
+  const uint32_t f = (Rsiz >> 8) & 0xFu;
+  return (f >= 1 && f <= 3) ? 2u : (f >= 4 && f <= 9) ? 1u : 0u;
+}
+
+void reduce_main_header(const std::vector<uint8_t>& hdr, const Params& in, uint32_t r, std::vector<uint8_t>& out,
+                        Params& outp) {
+  const uint32_t nc = in.num_comps();
+  // the levels: the decoder's own refusals of restrict_input_resolution (Decoder::restrict_resolution)
+  if (r > in.num_decomps)
+    fail(0x000300A2, "skipped_resolution for data %d must be smaller than  the number of decomposition levels %d",
+         r, in.num_decomps);
+  for (uint32_t c = 0; c < nc; ++c)
+    if (r > in.decomps(c))
+      fail(0x000B0007, "component %u has %u decomposition levels; %u cannot be skipped", c, in.decomps(c), r);
+  // a DFS level's split sets the reduction per direction and renumbers the kept bands' step-size entries
+  for (uint32_t c = 0; c < nc; ++c)
+    if (in.dfs_of(c) != nullptr)
+      fail(0x000B0054, "component %u uses a DFS decomposition structure: its resolutions cannot be dropped", c);
+  // SIZ: extent, image and tile offsets / 2^r rounded up; the tile size / 2^r along a direction with more than one
+  // tile (which must divide), else rounded up, which still covers the image.  Every tile must keep samples, so that
+  // tile indices -- and with them tile-parts and TLM entries -- stay the input's.
+  const uint64_t s = 1ull << r;
+  auto up = [&](uint32_t v) { return (uint32_t)(((uint64_t)v + s - 1) >> r); };
+  uint32_t tsz[2];
+  for (uint32_t d = 0; d < 2; ++d) {
+    const uint32_t X = d ? in.Ysiz : in.Xsiz, XO = d ? in.YOsiz : in.XOsiz, XT = d ? in.YTsiz : in.XTsiz,
+                   XTO = d ? in.YTOsiz : in.XTOsiz;
+    const uint32_t nt = (uint32_t)(((uint64_t)X - XTO + XT - 1) / XT);
+    if (nt > 1 && (XT & (s - 1)) != 0)
+      fail(0x000B0055, "the tile %s %u is not a multiple of 2^%u, and there is more than one tile along it",
+           d ? "height" : "width", XT, r);
+    const uint32_t X1 = up(X), XO1 = up(XO), XTO1 = up(XTO), XT1 = nt > 1 ? XT >> r : up(XT);
+    for (uint32_t k = 0; k < nt; ++k) {
+      const uint64_t a = std::max<uint64_t>((uint64_t)XTO1 + (uint64_t)k * XT1, XO1);
+      const uint64_t b = std::min<uint64_t>((uint64_t)XTO1 + (uint64_t)(k + 1) * XT1, X1);
+      if (a >= b)
+        fail(0x000B0055, "tile %s %u would be empty with %u resolution levels dropped", d ? "row" : "column", k, r);
+    }
+    tsz[d] = XT1;
+  }
+  // the step-size list a QCD serves: the components without a QCC
+  uint32_t qcd_levels = in.num_decomps;
+  for (uint32_t c = 0; c < nc; ++c)
+    if (!std::any_of(in.qcc.begin(), in.qcc.end(), [&](const QuantSet& q) { return q.comp_idx == c; }))
+      qcd_levels = std::max(qcd_levels, in.decomps(c));
+  const uint32_t cs = nc < 257 ? 1u : 2u;            // component index bytes of COC / QCC
+  out.assign(hdr.begin(), hdr.begin() + 2);          // SOC
+  size_t cap_at = 0;
+  for (size_t q = 2; q + 4 <= hdr.size(); ) {
+    const uint32_t m = ((uint32_t)hdr[q] << 8) | hdr[q + 1], L = ((uint32_t)hdr[q + 2] << 8) | hdr[q + 3];
+    std::vector<uint8_t> g(hdr.begin() + q, hdr.begin() + std::min(hdr.size(), q + 2 + L));
+    q += 2 + L;
+    auto put32 = [&](size_t o, uint32_t v) { g[o] = (uint8_t)(v >> 24); g[o + 1] = (uint8_t)(v >> 16); g[o + 2] = (uint8_t)(v >> 8); g[o + 3] = (uint8_t)v; };
+    auto cut = [&](size_t keep) {                   // the segment's first `keep` bytes, its length field to match
+      g.resize(keep);
+      g[2] = (uint8_t)((keep - 2) >> 8); g[3] = (uint8_t)(keep - 2);
+    };
+    if (m == M_SIZ && g.size() >= 40) {
+      put32(6, up(in.Xsiz)); put32(10, up(in.Ysiz)); put32(14, up(in.XOsiz)); put32(18, up(in.YOsiz));
+      put32(22, tsz[0]); put32(26, tsz[1]); put32(30, up(in.XTOsiz)); put32(34, up(in.YTOsiz));
+    } else if (m == M_CAP) {
+      cap_at = out.size();
+    } else if (m == M_COD && g.size() >= 14) {
+      g[9] = (uint8_t)(g[9] - r);                    // SPcod: decomposition levels
+      if (g[4] & 1) cut(g.size() - r);               // user precincts: entries 0 .. D - r
+    } else if (m == M_COC && g.size() >= 10 + cs) {
+      g[5 + cs] = (uint8_t)(g[5 + cs] - r);
+      if (g[4 + cs] & 1) cut(g.size() - r);
+    } else if ((m == M_QCD || m == M_QCC) && g.size() >= 5 + (m == M_QCC ? cs : 0)) {
+      const size_t h = 5 + (m == M_QCC ? cs : 0);    // marker, length, [component,] Sqcd
+      const uint32_t es = (g[h - 1] & 0x1F) == 0 ? 1u : 2u;
+      uint32_t levels = qcd_levels;
+      if (m == M_QCC) levels = in.decomps(cs == 1 ? g[4] : ((uint32_t)g[4] << 8) | g[5]);
+      // the bands are listed from the LL band up (get_Kmax / get_irrev_delta index (resolution - 1) * 3 + band): the
+      // kept ones are the first 1 + 3 (D - r), with the K_max and step size they had
+      const size_t n = (g.size() - h) / es, keep = std::min<size_t>(n, 1 + 3 * (levels - r));
+      cut(h + keep * es);
+    }
+    out.insert(out.end(), g.begin(), g.end());
+  }
+  // the reduced parameters as a decoder of the output reads them
+  std::vector<uint8_t> parse(out);
+  parse.push_back(0xFF); parse.push_back(0x90);
+  outp = Params();
+  outp.read_main_header(parse.data(), parse.size());
+  // CAP: MAGB of the cut step-size lists (the input's may overstate it)
+  if (cap_at) {
+    outp.Ccap0 = (uint16_t)((outp.Ccap0 & 0xFFE0) | outp.cap_magb());
+    out[cap_at + 8] = (uint8_t)(outp.Ccap0 >> 8); out[cap_at + 9] = (uint8_t)outp.Ccap0;
+  }
+  // a profile the input claims must hold for the output too (only its parameter rules: the tile-part division and
+  // TLM it would impose on an encoder stay the input's)
+  if (const uint32_t prof = claimed_profile(in.Rsiz)) {
+    Params pc = outp;
+    pc.profile = prof;
+    try { pc.check_profile(); }
+    catch (const Error& e) {
+      fail(0x000B0056, "the codestream claims the %s profile (Rsiz 0x%04X), which it would break with %u resolution "
+           "levels dropped: %s", prof == 1 ? "IMF" : "broadcast", in.Rsiz, r, e.what());
+    }
+  }
 }
 
 } // namespace ojb

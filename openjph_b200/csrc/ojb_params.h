@@ -221,11 +221,28 @@ struct Params {
 
   // finalisation before writing headers (write_headers, ojph_codestream_local.cpp:556-636)
   void finalize_for_encode();
+  // CAP's MAGB field (Ccap0 bits 0-4) for the QCD / QCC step-size lists
+  uint32_t cap_magb() const;
   void write_main_header(std::vector<uint8_t>& out, const char* const* comments,
                          const uint32_t* comment_lens, uint32_t n_comments) const;
   // decoder: parse from SOC up to (not including) the first SOT; returns offset of that SOT
   size_t read_main_header(const uint8_t* data, size_t len);
 };
+
+// The main header `hdr` (SOC up to the first SOT, without TLM / PLM) of a codestream with parameters `in`, rewritten
+// for the same codestream with its top r resolution levels dropped, and the parameters of that header.  Every kept
+// tile, resolution, band, precinct and code-block keeps its rectangle and its quantisation:
+//   SIZ      extent, image offset and tile offset / 2^r rounded up (ceil(ceil(a / b) / c) = ceil(a / (b c)), also with
+//            sub-sampling); the tile size / 2^r along a direction with several tiles, else rounded up
+//   COD/COC  r fewer levels; user precinct sizes 0 .. D_c - r
+//   QCD/QCC  the first 1 + 3 (D_c - r) step-size entries (they are indexed from the LL band up); guard bits and Sqcd kept
+//   CAP      MAGB recomputed from the cut lists
+// Every other segment is copied byte for byte.  Refused: r above some component's level count (0x000300A2, 0x000B0007,
+// as restrict_input_resolution), a DFS decomposition (0x000B0054), a tile grid whose tiles would not all keep samples
+// or whose tile size along a direction with several tiles is not a multiple of 2^r (0x000B0055), and a profile the
+// input's Rsiz claims that the reduced parameters break (0x000B0056).
+void reduce_main_header(const std::vector<uint8_t>& hdr, const Params& in, uint32_t r, std::vector<uint8_t>& out,
+                        Params& outp);
 
 // marker codes
 enum Marker : uint16_t {
